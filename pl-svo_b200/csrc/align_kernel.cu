@@ -7,7 +7,7 @@
 //   * per level: one thread issues a bulk async copy (TMA engine, cp.async.bulk -> UBLKCP) of the
 //     current image level into shared memory while all threads precompute the reference-patch
 //     cache (4x4 bilinear intensities + central-difference gradients: sparse_img_align.cpp:195-378)
-//     from the reference image in global memory into a per-CTA, L2-resident workspace.
+//     from the reference image in global memory into a per-CTA global workspace.
 //   * per GN pass, phase 1 (residuals): thread per patch.  The patch centre is warped in double, the
 //     4x4 residuals, robust weights and chi2 terms are evaluated in float with the reference's exact
 //     operation order (:450-500 points, :612-637 segment samples), and the five in-patch sums
@@ -41,6 +41,26 @@ namespace plsvo {
 namespace {
 
 constexpr int kOpqCap = 48;  // opaque patches (16 float terms each) per pass; one per binade crossing + margin
+
+#ifdef PLSVO_PHASE_CLOCKS
+// Opt-in cycle attribution (build_variant("phase", ["PLSVO_PHASE_CLOCKS"]), never the product build): lane 0 of every
+// warp adds the clock64() cycles since its previous mark to the phase the mark closes; the sums over the grid are read
+// with plsvo_phase_clocks() (tools/phase_clocks.py).  Every mark sits where its warp is converged.
+enum { kPhSetup, kPhPtEval, kPhPtChi2, kPhSeg, kPhReduce, kPhSerial, kPhPair, kNumPhases };
+__device__ unsigned long long g_phase_clocks[kNumPhases];
+#define PHASE_MARK(k)                      \
+  do {                                     \
+    if (lane == 0) {                       \
+      const long long now_ = clock64();    \
+      ph_acc[warp][k] += now_ - ph_t;      \
+      ph_t = now_;                         \
+    }                                      \
+  } while (0)
+#else
+#define PHASE_MARK(k) \
+  do {                \
+  } while (0)
+#endif
 
 struct PairCtl {
   double R[9];
@@ -212,17 +232,33 @@ __device__ __forceinline__ void rank2_update(double* acc, double xn, double yn, 
   for (int i = 0; i < 6; ++i) acc[21 + i] -= Sxr * r0[i] + Syr * r1[i];
 }
 
-// five consecutive image bytes starting at byte offset (sh/8) of the aligned word pair at `row`
-__device__ __forceinline__ void load_row5(const uint8_t* row, int sh, float* f) {
+// five consecutive image bytes starting at byte offset (sh/8) of the aligned word pair at `row`: bytes 0..3 in lo,
+// byte 4 in the low byte of hi.  They stay packed until used (row_px): two registers per footprint row instead of
+// five floats, which keeps the pass loop inside the 128-register budget of <128,4> with fewer spills.
+__device__ __forceinline__ void load_row5(const uint8_t* row, int sh, uint32_t& lo, uint32_t& hi) {
   const uint32_t w0 = *reinterpret_cast<const uint32_t*>(row);
   const uint32_t w1 = *reinterpret_cast<const uint32_t*>(row + 4);
-  const uint32_t lo = __funnelshift_r(w0, w1, sh);
-  const uint32_t hi = w1 >> sh;
-  f[0] = byte_to_float(lo, 0);
-  f[1] = byte_to_float(lo, 1);
-  f[2] = byte_to_float(lo, 2);
-  f[3] = byte_to_float(lo, 3);
-  f[4] = byte_to_float(hi, 0);
+  lo = __funnelshift_r(w0, w1, sh);
+  hi = w1 >> sh;
+}
+// pixel k (0..4, a compile-time constant after unrolling) of a row loaded by load_row5
+__device__ __forceinline__ float row_px(uint32_t lo, uint32_t hi, int k) {
+  return k < 4 ? byte_to_float(lo, k) : byte_to_float(hi, 0);
+}
+
+// (R*xyz_ref + t) / Z_ref for the point (xn, yn, zi) = (X/Z, Y/Z, 1/Z), projected into the current image at this
+// level (world2cam(xyz)*scale, :425).  The pass's pose is read from shared memory here, at each use: held in registers
+// across the pass it would take 24 of the 128 registers of <128,4> and push the accumulators into local memory.
+__device__ __forceinline__ void project(const PairCtl* ctl, const AlignArgs& a, double dscale, double xn, double yn,
+                                        double zi, double& u, double& v) {
+  const double* R = ctl->R;
+  const double* t = ctl->t;
+  const double xc = R[0] * xn + R[1] * yn + (R[2] + t[0] * zi);
+  const double yc = R[3] * xn + R[4] * yn + (R[5] + t[1] * zi);
+  const double zc = R[6] * xn + R[7] * yn + (R[8] + t[2] * zi);
+  const double izc = __drcp_rn(zc);
+  u = (a.fx * (xc * izc) + a.cx) * dscale;
+  v = (a.fy * (yc * izc) + a.cy) * dscale;
 }
 // seven consecutive bytes (reference image, global memory, read-only path)
 __device__ __forceinline__ void load_row7(const uint8_t* row, int sh, float* g) {
@@ -259,8 +295,8 @@ __device__ __forceinline__ bool eval_patch(const uint8_t* __restrict__ img, int 
   const int c0 = ui - 2;
   const int sh = (c0 & 3) * 8;
   const uint8_t* rowp = img + (size_t)(vi - 2) * pitch + (c0 & ~3);
-  float ra[5], rb[5];
-  load_row5(rowp, sh, ra);
+  uint32_t ra_lo, ra_hi, rb_lo, rb_hi;
+  load_row5(rowp, sh, ra_lo, ra_hi);
 #ifdef PLSVO_FP32_SUMS
   float Sxx = 0.f, Sxy = 0.f, Syy = 0.f, Sxr = 0.f, Syr = 0.f;
 #else
@@ -271,7 +307,7 @@ __device__ __forceinline__ bool eval_patch(const uint8_t* __restrict__ img, int 
 #pragma unroll 1
   for (int y = 0; y < 4; ++y) {
     rowp += pitch;
-    load_row5(rowp, sh, rb);
+    load_row5(rowp, sh, rb_lo, rb_hi);
     const float4 ref4 = cp[0];
     const float4 dx4 = cp[4 * MP];
     const float4 dy4 = cp[8 * MP];
@@ -281,7 +317,8 @@ __device__ __forceinline__ bool eval_patch(const uint8_t* __restrict__ img, int 
     const float dyv[4] = {dy4.x, dy4.y, dy4.z, dy4.w};
 #pragma unroll
     for (int x = 0; x < 4; ++x) {
-      const float cur = bilin(wTL, wTR, wBL, wBR, ra[x], ra[x + 1], rb[x], rb[x + 1]);
+      const float cur = bilin(wTL, wTR, wBL, wBR, row_px(ra_lo, ra_hi, x), row_px(ra_lo, ra_hi, x + 1),
+                              row_px(rb_lo, rb_hi, x), row_px(rb_lo, rb_hi, x + 1));
       const float res = __fsub_rn(cur, refv[x]);
       const float dx = dxv[x], dy = dyv[x];
       const float ares = fabsf(res);
@@ -308,8 +345,7 @@ __device__ __forceinline__ bool eval_patch(const uint8_t* __restrict__ img, int 
       Syr = fma(-nwdy, rd, Syr);
 #endif
     }
-#pragma unroll
-    for (int c = 0; c < 5; ++c) ra[c] = rb[c];
+    ra_lo = rb_lo, ra_hi = rb_hi;
   }
   S[0] = (double)Sxx, S[1] = (double)Sxy, S[2] = (double)Syy, S[3] = (double)Sxr, S[4] = (double)Syr;
   tsum = acc_f;  // fl-sum of the 16 (positive) terms started from zero: the estimate of this patch's contribution
@@ -512,7 +548,7 @@ __global__ void __launch_bounds__(NT, MINB) sparse_img_align_kernel(const AlignA
   float* seg_term = reinterpret_cast<float*>(smem + L.seg_term);
   uint8_t* pt_vis = smem + L.pt_vis;
   uint8_t* img_s = smem + L.img;
-  // per-CTA workspaces in global memory (L2 resident)
+  // per-CTA workspaces in global memory
   float4* cache = a.ws_cache + (size_t)blockIdx.x * kCacheRows * MP;
   double* xyz = reinterpret_cast<double*>(smem + L.xyz);
   float* tsc = reinterpret_cast<float*>(smem + L.tsc) + tid;  // this thread's term k at tsc[k * NT]
@@ -528,6 +564,12 @@ __global__ void __launch_bounds__(NT, MINB) sparse_img_align_kernel(const AlignA
   }
   __syncthreads();
   uint32_t bar_parity = 0;
+#ifdef PLSVO_PHASE_CLOCKS
+  __shared__ unsigned long long ph_acc[NW][kNumPhases];
+  if (lane == 0)
+    for (int k = 0; k < kNumPhases; ++k) ph_acc[warp][k] = 0ull;
+  long long ph_t = clock64();
+#endif
 
   for (;;) {
     __syncthreads();  // everyone is done with ctl of the previous pair
@@ -640,6 +682,7 @@ __global__ void __launch_bounds__(NT, MINB) sparse_img_align_kernel(const AlignA
     const int rounds = (np + NT - 1) / NT;     // rounds of NT point patches per pass
 
     for (int level = a.max_level; level >= a.min_level; --level) {
+      PHASE_MARK(kPhPair);
       const int cols = a.width >> level, rows = a.height >> level;
       const int pitch = (int)a.pitch[level];
       const float scale = 1.0f / (float)(1 << level);
@@ -805,14 +848,12 @@ __global__ void __launch_bounds__(NT, MINB) sparse_img_align_kernel(const AlignA
         bar_parity ^= 1u;
       }
       __syncthreads();
+      PHASE_MARK(kPhSetup);
 
       // ---- Gauss-Newton iterations at this level (vk::NLLSSolver::optimizeGaussNewton) ----
       const double cJ = fabs(a.fx) / (double)(1 << level);  // focal_length / 2^level (:262)
       const double cJ2 = cJ * cJ;
       for (;;) {
-        const double R0 = ctl->R[0], R1 = ctl->R[1], R2 = ctl->R[2], R3 = ctl->R[3], R4 = ctl->R[4], R5 = ctl->R[5],
-                     R6 = ctl->R[6], R7 = ctl->R[7], R8 = ctl->R[8];
-        const double t0 = ctl->t[0], t1 = ctl->t[1], t2 = ctl->t[2];
         int n_meas_acc = 0, n_patch_acc = 0;
 #ifdef PLSVO_TREE_CHI2
         double chi2_tree = 0.0;
@@ -830,12 +871,8 @@ __global__ void __launch_bounds__(NT, MINB) sparse_img_align_kernel(const AlignA
           bool ok = false;
           if (p < np && pt_vis[p]) {
             const double xn = xyz[0 * MP + p], yn = xyz[1 * MP + p], zi = xyz[2 * MP + p];
-            const double xc = R0 * xn + R1 * yn + (R2 + t0 * zi);  // (R*xyz_ref + t) / Z_ref
-            const double yc = R3 * xn + R4 * yn + (R5 + t1 * zi);
-            const double zc = R6 * xn + R7 * yn + (R8 + t2 * zi);
-            const double izc = __drcp_rn(zc);
-            const double u = (a.fx * (xc * izc) + a.cx) * dscale;  // world2cam(xyz)*scale (:425)
-            const double v = (a.fy * (yc * izc) + a.cy) * dscale;
+            double u, v;
+            project(ctl, a, dscale, xn, yn, zi, u, v);
             double S[5];
             ok = eval_patch<true, NT>(cur_img, pitch, cols, rows, cache, MP, p, u, v, S, tsc, Tf);
             if (ok) {
@@ -846,6 +883,7 @@ __global__ void __launch_bounds__(NT, MINB) sparse_img_align_kernel(const AlignA
             }
           }
           if (!ok) Tf = 0.f;  // not evaluated: contributes nothing (its scratch terms are stale and never read)
+          PHASE_MARK(kPhPtEval);
 #ifdef PLSVO_TREE_CHI2
           chi2_tree += (double)Tf;
 #else
@@ -853,6 +891,7 @@ __global__ void __launch_bounds__(NT, MINB) sparse_img_align_kernel(const AlignA
             // a warp whose chunk lies beyond the point list (last round only) signals the round barrier without waiting
             // and goes on to its segment rounds: it needs none of the totals the others are about to exchange
             named_barrier_arrive(2, NT);
+            PHASE_MARK(kPhPtChi2);
             continue;
           }
           // -- estimate of the accumulator before this patch: exact prefix sum of the patch totals --
@@ -932,6 +971,7 @@ __global__ void __launch_bounds__(NT, MINB) sparse_img_align_kernel(const AlignA
             if (lane == 0) item_cnt[c] = __popc(tails);
           }
 #endif
+          PHASE_MARK(kPhPtChi2);
         }
         // ======== segment samples (:504-695).  Every segment owns a group of G = 2^k consecutive lanes of one warp
         // (G >= its sample count, or the whole warp looping over samples), so the per-segment gate / weight
@@ -967,13 +1007,8 @@ __global__ void __launch_bounds__(NT, MINB) sparse_img_align_kernel(const AlignA
             bool ok = false;
             if (active) {
               p = np + off + n;
-              const double xn = xyz[0 * MP + p], yn = xyz[1 * MP + p], zi = xyz[2 * MP + p];
-              const double xc = R0 * xn + R1 * yn + (R2 + t0 * zi);
-              const double yc = R3 * xn + R4 * yn + (R5 + t1 * zi);
-              const double zc = R6 * xn + R7 * yn + (R8 + t2 * zi);
-              const double izc = __drcp_rn(zc);
-              const double u = (a.fx * (xc * izc) + a.cx) * dscale;
-              const double v = (a.fy * (yc * izc) + a.cy) * dscale;
+              double u, v;
+              project(ctl, a, dscale, xyz[0 * MP + p], xyz[1 * MP + p], xyz[2 * MP + p], u, v);
               ok = eval_patch<false, NT>(cur_img, pitch, cols, rows, cache, MP, p, u, v, S, tsc, Tf);
               if (ok) {
                 ok_trips |= 1u << (trip & 31);
@@ -1043,6 +1078,7 @@ __global__ void __launch_bounds__(NT, MINB) sparse_img_align_kernel(const AlignA
             }
           }
         }
+        PHASE_MARK(kPhSeg);
         acc[28] = (double)n_meas_acc;
         acc[29] = (double)n_patch_acc;
 #ifdef PLSVO_TREE_CHI2
@@ -1052,6 +1088,7 @@ __global__ void __launch_bounds__(NT, MINB) sparse_img_align_kernel(const AlignA
         const double mine = warp_reduce32(acc, lane);
         red[warp * 32 + lane] = mine;
         __syncthreads();
+        PHASE_MARK(kPhReduce);
         if (warp == 0) {
           double s = 0.0;
 #pragma unroll
@@ -1146,6 +1183,7 @@ __global__ void __launch_bounds__(NT, MINB) sparse_img_align_kernel(const AlignA
         if (tid == 0) gn_decide(ctl, tot, __fadd_rn(ctl->chi2f, ctl->seg_chi2f), a.n_iter, a.eps);  // pt_chi2 + seg_chi2 (:171)
 #endif
         __syncthreads();
+        PHASE_MARK(kPhSerial);
         if (ctl->flag) break;
       }
     }  // levels
@@ -1180,6 +1218,11 @@ __global__ void __launch_bounds__(NT, MINB) sparse_img_align_kernel(const AlignA
       a.out_patch_levels[b] = ctl->patch_levels;
     }
   }
+#ifdef PLSVO_PHASE_CLOCKS
+  PHASE_MARK(kPhPair);
+  if (lane == 0)
+    for (int k = 0; k < kNumPhases; ++k) atomicAdd(&g_phase_clocks[k], ph_acc[warp][k]);
+#endif
 }
 
 }  // namespace
@@ -1255,3 +1298,17 @@ cudaError_t align_kernel_launch(const AlignArgs& a, int grid, int threads, int m
 }
 
 }  // namespace plsvo
+
+#ifdef PLSVO_PHASE_CLOCKS
+// per-phase cycle sums of sparse_img_align_kernel since the last reset, in the order of the kPh* enum (7 values);
+// reset != 0 zeroes them afterwards.  Synchronous.  Only in -DPLSVO_PHASE_CLOCKS builds.
+extern "C" int plsvo_phase_clocks(unsigned long long* out, int reset) {
+  cudaError_t e = cudaDeviceSynchronize();
+  if (e == cudaSuccess) e = cudaMemcpyFromSymbol(out, plsvo::g_phase_clocks, sizeof(plsvo::g_phase_clocks));
+  if (e == cudaSuccess && reset) {
+    const unsigned long long zero[plsvo::kNumPhases] = {};
+    e = cudaMemcpyToSymbol(plsvo::g_phase_clocks, zero, sizeof(zero));
+  }
+  return (int)e;
+}
+#endif

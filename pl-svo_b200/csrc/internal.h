@@ -60,7 +60,7 @@ struct AlignArgs {
   int max_seg_patches;  // segment sample slots per pair
   int max_seg_slots;    // lane slots of the segment groups per pair (multiple of 32)
   int smem_img_bytes;   // bytes of the image staging buffer
-  float4* ws_cache;     // [grid][kCacheRows][max_patches] reference-patch cache (ref, dx, dy rows), L2 resident
+  float4* ws_cache;     // [grid][kCacheRows][max_patches] reference-patch cache (ref, dx, dy rows)
   double* ws_segpx;     // [grid][2][max_seg_patches] 2-D centre of every segment sample (precompute only)
   double* ws_rec;       // [grid][5][rec_cap*threads] parked in-patch sums of segments longer than a warp
   int rec_cap;          // 32-sample trips of the longest segment, <= 32

@@ -868,7 +868,7 @@ int align_plan(plsvo_ctx_impl* c, const plsvo_align_params* p, int chunk_pairs, 
     }
     const char* cap = getenv("PLSVO_CTAS_PER_SM");
     if (cap && atoi(cap) > 0) ctas_per_sm = std::min(ctas_per_sm, atoi(cap));
-    // per-CTA workspaces (L2 resident): reference-patch cache, patch geometry, segment sample centres, pass records
+    // per-CTA workspaces: reference-patch cache, patch geometry, segment sample centres, pass records
     const size_t grid_max = (size_t)std::min(a.B, c->num_sms * ctas_per_sm);
     CK(ensure(c->d_ws_cache, grid_max * kCacheRows * a.max_patches * sizeof(float4)));
     CK(ensure(c->d_ws_segpx, grid_max * 2 * a.max_seg_patches * sizeof(double)));
