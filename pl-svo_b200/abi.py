@@ -242,6 +242,11 @@ def _ptr(a, dtype):
     return a.ctypes.data_as(_CT[np.dtype(dtype)])
 
 
+# Compiled variants of the alignment kernel as (threads per CTA, resident CTAs per SM), the values PLSVO_VARIANT accepts
+# ("threads,ctas"): kAlignVariants in csrc/plsvo_abi.cu.  A variant missing here is missing from the parity tests.
+ALIGN_VARIANTS = ((64, 8), (96, 7), (96, 5), (128, 5), (128, 4), (160, 3), (192, 2), (256, 2))
+
+
 def align_params(max_level=4, min_level=2, n_iter=30, eps=1e-6) -> AlignParams:
     return AlignParams(max_level, min_level, n_iter, 0, eps)
 

@@ -40,8 +40,6 @@ namespace plsvo {
 
 namespace {
 
-constexpr int kOpqCap = 48;  // opaque patches (16 float terms each) per pass; one per binade crossing + margin
-
 #ifdef PLSVO_PHASE_CLOCKS
 // Opt-in cycle attribution (build_variant("phase", ["PLSVO_PHASE_CLOCKS"]), never the product build): lane 0 of every
 // warp adds the clock64() cycles since its previous mark to the phase the mark closes; the sums over the grid are read
@@ -122,8 +120,6 @@ __host__ __device__ inline Layout make_layout(int n_pts, int n_segs, int max_pat
   o += 4u * (n_chunks + 1u);
   L.flat = align_up(o, 8);
   o = L.flat + 8u * 64u;  // the walker's current batch of items, in list order
-  L.opq = align_up(o, 16);
-  o = L.opq + 64u * (uint32_t)kOpqCap;
   L.seg_N0 = o;
   o += 4u * (uint32_t)n_segs;  // samples of every segment at level 0 (setupSampling), once per pair
   L.seg_N = o;
@@ -148,6 +144,8 @@ __host__ __device__ inline Layout make_layout(int n_pts, int n_segs, int max_pat
   o = align_up(o, 128);
   L.img = o;
   o += (uint32_t)img_bytes + 16u;  // slack: the 5-byte row reads fetch whole aligned words
+  L.opq = align_up(o, 16);         // last: the only region whose size depends on the point count's square
+  o = L.opq + 64u * (uint32_t)align_opq_cap(n_pts);
   L.total = o;
   return L;
 }
@@ -512,12 +510,13 @@ __device__ __forceinline__ void named_barrier_arrive(int id, int nthreads) {
   asm volatile("bar.arrive %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
 }
 
-// ---- chi2 items (shared memory, 8 bytes): x = A_even (ulps added when the running sum's mantissa is even),
-// y = [15:0] A_odd - A_even (signed) | [23:16] biased float exponent of the binade | [24] opaque | [31:25] opaque slot
+// ---- chi2 items (shared memory, 8 bytes): x = A_even (ulps added when the running sum's mantissa is even), or the
+// opaque slot of an opaque patch (whose map is never read); y = [15:0] A_odd - A_even (signed) | [23:16] biased float
+// exponent of the binade | [24] opaque
 __device__ __forceinline__ uint2 make_item(uint32_t Ae, uint32_t Ao, uint32_t ef, uint32_t opaque, uint32_t slot) {
   uint2 it;
-  it.x = Ae;
-  it.y = ((Ao - Ae) & 0xffffu) | (ef << 16) | (opaque << 24) | (slot << 25);
+  it.x = Ae | slot;  // one of them is 0
+  it.y = ((Ao - Ae) & 0xffffu) | (ef << 16) | (opaque << 24);
   return it;
 }
 
@@ -918,13 +917,14 @@ __global__ void __launch_bounds__(NT, MINB) sparse_img_align_kernel(const AlignA
             const double lo = P * (1.0 - delta), hi = (P + (double)Tf) * (1.0 + delta);
             const int e_lo = (__double2hiint(lo) >> 20) - 1023, e_hi = (__double2hiint(hi) >> 20) - 1023;
             uint32_t ef = 0, opaque = 0, Ae = 0, Ao = 0, slot = 0;
-            if (!ok) {
-              // no terms: identity map.  It joins the binade of the estimate so that it merges with its neighbours
-              // (P == 0: still in front of the first non-zero term).
+            if (Tf == 0.f) {
+              // not evaluated (Tf was zeroed above), or 16 terms that are all +0 (the terms are never negative, so Tf == 0
+              // means exactly that): identity map, never opaque, wherever the estimate lies.  It joins the binade of the
+              // estimate so that it merges with its neighbours (P == 0: still in front of the first non-zero term).
               if (P != 0.0 && e_lo == e_hi && e_lo >= -100 && e_lo <= 100) ef = (uint32_t)(e_lo + 127);
               else if (P != 0.0) ef = 255u;  // next to a power of two: a group of its own, still the identity
             } else if (P == 0.0) {
-              opaque = (Tf != 0.f) ? 1u : 0u;  // leading zeros leave the accumulator at 0
+              opaque = 1u;  // the first non-zero patch: leading zeros leave the accumulator at 0
             } else if (e_lo != e_hi || e_lo < -100 || e_lo > 100) {
               opaque = 1u;
             } else {
@@ -938,7 +938,7 @@ __global__ void __launch_bounds__(NT, MINB) sparse_img_align_kernel(const AlignA
             }
             if (opaque) {
               const int idx = atomicAdd(&ctl->n_opq, 1);
-              if (idx < kOpqCap) {
+              if (idx < align_opq_cap(a.n_pts)) {
                 slot = (uint32_t)idx;
 #pragma unroll
                 for (int k = 0; k < 16; ++k) opq[idx * 16 + k] = tsc[k * NT];
@@ -1128,7 +1128,7 @@ __global__ void __launch_bounds__(NT, MINB) sparse_img_align_kernel(const AlignA
               if (b0 + lane < total) it = flat[b0 + lane];
               float4 q0 = make_float4(0.f, 0.f, 0.f, 0.f), q1 = q0, q2 = q0, q3 = q0;
               if ((it.y >> 24) & 1u) {  // this lane's item is an opaque patch: fetch its 16 terms now, off the chain
-                const float4* o4 = reinterpret_cast<const float4*>(opq + (it.y >> 25) * 16);
+                const float4* o4 = reinterpret_cast<const float4*>(opq + it.x * 16);
                 q0 = o4[0], q1 = o4[1], q2 = o4[2], q3 = o4[3];
               }
               const float tr[16] = {q0.x, q0.y, q0.z, q0.w, q1.x, q1.y, q1.z, q1.w, q2.x, q2.y, q2.z, q2.w, q3.x, q3.y, q3.z, q3.w};
@@ -1157,7 +1157,7 @@ __global__ void __launch_bounds__(NT, MINB) sparse_img_align_kernel(const AlignA
             c += nfit;
           }
           if (lane == 0) {
-            if (ctl->n_opq > kOpqCap) {
+            if (ctl->n_opq > align_opq_cap(a.n_pts)) {
               // opaque buffer overflowed (flag 1): fall back to the estimate of the point sum for this pass
               double e = 0.0;
               for (int c = 0; c < n_chunks; ++c) e += chunk_tot[c];
@@ -1211,8 +1211,8 @@ __global__ void __launch_bounds__(NT, MINB) sparse_img_align_kernel(const AlignA
       a.out_n_tracked[b] = ctl->n_meas_last / 16;  // :94
       for (int i = 0; i < 36; ++i) a.out_H[(size_t)b * 36 + i] = ctl->H_last[i];
       for (int l = 0; l < PLSVO_MAX_LEVELS; ++l) a.out_iters[(size_t)b * PLSVO_MAX_LEVELS + l] = ctl->iters_level[l];
-      // status: bit 1 = solver stopped (NaN step); bits 2,3 = chi2 order could not be reproduced exactly (never
-      // seen in practice; kept loud instead of silent)
+      // status: bit 1 = solver stopped (NaN step); bits 2,3 = chi2 order could not be reproduced exactly (not raised
+      // by the parity suite, which reaches 4096 points per pair; kept loud instead of silent)
       a.out_status[b] = (ctl->stop ? 2 : 0) | (ctl->chi2_flags << 2);
       a.out_patch_iters[b] = ctl->patch_iters;
       a.out_patch_levels[b] = ctl->patch_levels;

@@ -67,6 +67,13 @@ struct AlignArgs {
   int derive_from;      // >= 0: the CTA forms levels (derive_from, max_level] of its pair by halfSample (gated pipeline)
 };
 
+// Opaque chi2 patches (16 float terms each) the alignment kernel can hold per Gauss-Newton pass: the patches whose 16
+// additions may carry the float accumulator across a power of two, chained term by term.  The classification margin
+// grows with the patch index, so their number grows with the square of the point count; this leaves at least a factor
+// of two over the count the exact-order model of tests/test_chi2_order_cpu.py gives, at every point count shared memory
+// admits.  A pass that still overflows it flags status bit 2 and approximates the chi2.
+__host__ __device__ inline int align_opq_cap(int n_pts) { return 48 + (int)((long long)n_pts * n_pts / 131072); }
+
 // shared memory the kernel needs for a configuration (host + device agree through this)
 size_t align_smem_bytes(int n_pts, int n_segs, int max_patches, int max_seg_slots, int img_bytes, int threads);
 // kernel variants are compiled per (threads per CTA, resident CTAs per SM the register budget allows):

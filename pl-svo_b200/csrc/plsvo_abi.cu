@@ -807,27 +807,29 @@ int align_plan(plsvo_ctx_impl* c, const plsvo_align_params* p, int chunk_pairs, 
 
   // Kernel variant.  Default: 128-thread CTAs with the register budget of four resident pairs per SM; small
   // batches (at most one pair per SM) take 256-thread CTAs to cut the latency of a pair.
-  // PLSVO_VARIANT="threads,ctas" selects another compiled variant (tuning and A/B runs).
+  // PLSVO_VARIANT="threads,ctas" selects another compiled variant (tuning, A/B runs, tests).  A selected variant is the
+  // only one tried: a batch it cannot run is an error, so whoever selected it knows which kernel ran.
   int want_t = 128, want_b = 4;
   if (chunk_pairs <= c->num_sms) want_t = 256, want_b = 2;
   // streamed host path: pairs trickle in at the rate of the host link, so fewer are in flight than the grid has room for
   // and the call ends one pair-latency after the last chunk lands — bigger CTAs shorten that tail (tools/e2e_trace.py)
   else if (streamed) want_t = 192, want_b = 2;
-  if (const char* v = getenv("PLSVO_VARIANT")) {
+  const char* forced = getenv("PLSVO_VARIANT");
+  if (forced && !*forced) forced = nullptr;
+  if (forced) {
     int t = 0, mb = 0;
-    if (sscanf(v, "%d,%d", &t, &mb) == 2) {
-      bool known = false;
-      for (auto& kv : kAlignVariants) known |= (kv[0] == t && kv[1] == mb);
-      if (!known) return fail(c, PLSVO_ERR_INVALID, "PLSVO_VARIANT names a variant that is not compiled");
-      want_t = t, want_b = mb;
-    }
+    if (sscanf(forced, "%d,%d", &t, &mb) != 2) return fail(c, PLSVO_ERR_INVALID, "PLSVO_VARIANT is not of the form \"threads,ctas\"");
+    bool known = false;
+    for (auto& kv : kAlignVariants) known |= (kv[0] == t && kv[1] == mb);
+    if (!known) return fail(c, PLSVO_ERR_INVALID, "PLSVO_VARIANT names a variant that is not compiled");
+    want_t = t, want_b = mb;
   }
   const int limit = c->smem_optin;  // 227 KB on sm_90a
   // try the wanted variant first, then bigger CTAs (more patches per round, fewer records per thread)
   const int order[][2] = {{want_t, want_b}, {128, 4}, {256, 2}};
   int rc_last = PLSVO_ERR_INVALID;
-  for (auto& v : order) {
-    const int threads = v[0], min_blocks = v[1];
+  for (int i = 0; i < (forced ? 1 : 3); ++i) {
+    const int threads = order[i][0], min_blocks = order[i][1];
     // parked in-patch sums of a segment longer than a warp (one record per thread and 32-sample trip)
     const int rec_cap = std::max(1, (maxN + 31) / 32);
     if (rec_cap > 32) {
@@ -878,6 +880,12 @@ int align_plan(plsvo_ctx_impl* c, const plsvo_align_params* p, int chunk_pairs, 
     a.ws_rec = static_cast<double*>(c->d_ws_rec.p);
     plan->threads = threads, plan->min_blocks = min_blocks, plan->ctas_per_sm = ctas_per_sm, plan->smem = smem;
     return PLSVO_OK;
+  }
+  if (forced) {
+    const std::string why = c->err;
+    char msg[128];
+    snprintf(msg, sizeof msg, "PLSVO_VARIANT=%d,%d cannot run this batch: ", want_t, want_b);
+    return fail(c, rc_last, (msg + why).c_str());
   }
   return rc_last;
 }

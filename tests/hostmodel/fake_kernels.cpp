@@ -263,7 +263,7 @@ size_t align_smem_bytes(int n_pts, int n_segs, int max_patches, int max_seg_slot
   size_t o = 1024;                                   // control block
   o += nw * 256 + 256 + 8 * (rounds * nw + 1);       // reduction scratch, chunk totals
   o += 256 * (chunks + 1) + 4 * (chunks + 1) + 512;  // chi2 items
-  o += 64 * 48;                                      // opaque patches
+  o += 64 * (size_t)align_opq_cap(n_pts);            // opaque patches
   o += 21 * (size_t)n_segs + 2 * (size_t)max_seg_slots + (size_t)n_pts;
   o += 24 * (size_t)max_patches + 64 * (size_t)threads;
   o = (o + 127) / 128 * 128;

@@ -374,6 +374,42 @@ def s_rejected_inputs_leave_nothing_in_flight():
     check(run(ok, ctx=ctx), ok, "after rejected calls")
 
 
+def s_forced_variant_is_the_only_one_tried():
+    """PLSVO_VARIANT selects the one kernel variant a call may run: a batch that variant cannot plan fails and names it,
+    while the default plan of the same batch falls back to a variant that fits."""
+    ctx = pkg.api.Context(0)
+
+    def fits(n_pts, variant):
+        d = make_batch(1, n_pts, 0, 160)
+        try:
+            out = run(d, ctx=ctx, PLSVO_VARIANT=variant)
+        except pkg.api.PlsvoError as ex:
+            assert f"PLSVO_VARIANT={variant} cannot run this batch" in str(ex) and "shared-memory plan" in str(ex), str(ex)
+            clean()
+            return False
+        check(out, d, f"{variant}, {n_pts} points")
+        return True
+
+    # <256,2> needs more shared memory per point list than <128,4> (per-thread chi2 terms, cross-warp partials): find the
+    # smallest point count it cannot plan
+    lo, hi = 1000, 8000
+    assert fits(lo, "256,2") and not fits(hi, "128,4")
+    while hi - lo > 1:
+        mid = (lo + hi) // 2
+        lo, hi = (mid, hi) if fits(mid, "256,2") else (lo, mid)
+    assert fits(hi, "128,4"), f"{hi} points: <128,4> should still fit where <256,2> stops"
+    d = make_batch(1, hi, 0, 161)
+    check(run(d, ctx=ctx), d, f"default plan of one pair (<256,2> first), {hi} points")
+    for bad, why in (("128,3", "not compiled"), ("128x4", "threads,ctas")):
+        try:
+            run(make_batch(1, 10, 2, 162), ctx=ctx, PLSVO_VARIANT=bad)
+        except pkg.api.PlsvoError as ex:
+            assert why in str(ex), str(ex)
+        else:
+            raise AssertionError(f"PLSVO_VARIANT={bad} was accepted")
+    clean()
+
+
 def poseopt_expected(po, T=None):
     B = po.batch
     want = np.zeros(B, np.uint64)

@@ -104,3 +104,15 @@ def test_numa_helper_degrades_to_a_no_op_without_a_gpu():
     assert os.sched_getaffinity(0) == before
     d = numa.describe(0)
     assert set(d) == {"pci_bus_id", "numa_node", "local_cpus", "process_cpus"}
+
+
+def test_align_variant_list_matches_the_compiled_variants(abi):
+    """abi.ALIGN_VARIANTS is what the parity tests iterate over: it must name every variant the library compiles and
+    the planner accepts, no more and no fewer."""
+    csrc = os.path.join(ROOT, "pl-svo_b200", "csrc")
+    kernel = open(os.path.join(csrc, "align_kernel.cu")).read()
+    compiled = re.search(r"#define PLSVO_ALIGN_VARIANTS\(X\)(.*)", kernel).group(1)
+    plan = re.search(r"kAlignVariants\[\]\[2\] = \{(.*)\};", open(os.path.join(csrc, "plsvo_abi.cu")).read()).group(1)
+    want = sorted(abi.ALIGN_VARIANTS)
+    assert sorted((int(t), int(b)) for t, b in re.findall(r"X\((\d+), (\d+)\)", compiled)) == want
+    assert sorted((int(t), int(b)) for t, b in re.findall(r"\{(\d+), (\d+)\}", plan)) == want

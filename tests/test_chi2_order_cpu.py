@@ -33,9 +33,15 @@ def from_bits(b):
     return np.array([b & 0xFFFFFFFF], dtype=np.uint32).view(np.float32)[0]
 
 
-def kernel_model(terms, nt=128, opq_cap=48):
+def align_opq_cap(n_pts):
+    """Opaque slots per pass of a batch with n_pts points: align_opq_cap, pl-svo_b200/csrc/internal.h."""
+    return 48 + n_pts * n_pts // 131072
+
+
+def kernel_model(terms, nt=128, opq_cap=None):
     """terms: [np, 16] float32 >= 0.  Returns (float32 sum, number of opaque patches)."""
     n_p = terms.shape[0]
+    opq_cap = align_opq_cap(n_p) if opq_cap is None else opq_cap
     nw = nt // 32
     rounds = (n_p + nt - 1) // nt
     n_chunks = (n_p + 31) // 32
@@ -69,8 +75,14 @@ def kernel_model(terms, nt=128, opq_cap=48):
                 lo, hi = P * (1.0 - delta), (P + float(Tf)) * (1.0 + delta)
                 ef = Ae = Ao = 0
                 opaque = False
-                if P == 0.0:
-                    opaque = Tf != 0
+                if Tf == 0:
+                    # no terms, or 16 terms that are all +0: the identity, never opaque.  It takes the estimate's binade,
+                    # or a group of its own (255) next to a power of two.
+                    if P != 0.0:
+                        e_lo, e_hi = int(np.floor(np.log2(lo))), int(np.floor(np.log2(hi)))
+                        ef = e_lo + 127 if e_lo == e_hi and -100 <= e_lo <= 100 else 255
+                elif P == 0.0:
+                    opaque = True
                 else:
                     e_lo, e_hi = int(np.floor(np.log2(lo))), int(np.floor(np.log2(hi)))
                     if e_lo != e_hi or e_lo < -100 or e_lo > 100:
@@ -103,7 +115,7 @@ def kernel_model(terms, nt=128, opq_cap=48):
         for it in items[c]:
             if it[0] == "opq":
                 s = chain16(s, it[1])
-            else:
+            elif it[1] != 0 or it[2] != it[1]:  # the walker skips identity maps
                 b = bits(s)
                 assert (b >> 23) == it[3] or (it[3] == 0 and b == 0), "binade check"
                 assert abs(it[2] - it[1]) < 32768
@@ -170,3 +182,44 @@ def test_exact_order_growing_magnitudes():
     got, n_opq = kernel_model(terms, 128)
     assert bits(got) == bits(seq_sum(terms))
     assert n_opq <= 48
+
+
+# More points than this cannot fit in the 227 KB of shared memory of an sm_90a CTA, whatever the variant and the segments:
+# every point takes at least 33 bytes of it (its 3-D point, 24; its chi2 item, 8; its visibility, 1; make_layout).
+MAX_PTS_SMEM = 232448 // 33
+
+
+@pytest.mark.parametrize("nt", [64, 96, 128, 160, 192, 256])
+@pytest.mark.parametrize("n_p", [2048, 4096, MAX_PTS_SMEM])
+def test_opaque_buffer_scales_with_the_point_count(n_p, nt):
+    """The classification margin grows with the patch index, so the opaque patches grow with the square of the point
+    count: at 4096 residual-like patches there are more than the 48 slots the buffer once had.  The sized buffer keeps
+    a factor of two in hand, and the sum stays the sequential one bit for bit."""
+    rng = np.random.default_rng(n_p + nt)
+    worst = 0
+    for trial in range(2):
+        terms = _residual_like(rng, n_p)
+        got, n_opq = kernel_model(terms, nt)
+        assert bits(got) == bits(seq_sum(terms)), (trial, float(got))
+        assert n_opq <= align_opq_cap(n_p) // 2, (trial, n_opq, align_opq_cap(n_p))
+        worst = max(worst, n_opq)
+    if n_p >= 4096:
+        assert worst > 48  # what a fixed buffer of 48 slots could not hold
+
+
+def test_zero_patches_next_to_a_power_of_two_are_not_opaque():
+    """80 evaluated patches whose terms are all +0, right below a power of two: they are the identity and take no
+    opaque slot, so the list has no more opaque patches than without them."""
+    rng = np.random.default_rng(1)
+    terms = _residual_like(rng, 600)
+    k = 250
+    before = terms[:k].astype(np.float64).sum()
+    terms[k] = F((2.0 ** np.ceil(np.log2(before)) * (1 - 1e-5) - before) / 16)  # the sum ends just below 2^e
+    without = np.delete(terms, np.s_[k + 1:k + 81], axis=0)
+    terms[k + 1:k + 81] = 0
+    for nt in (64, 128, 256):
+        got, n_opq = kernel_model(terms, nt)
+        assert bits(got) == bits(seq_sum(terms))
+        got0, n_opq0 = kernel_model(without, nt)
+        assert bits(got0) == bits(got)
+        assert n_opq <= n_opq0, (nt, n_opq, n_opq0)

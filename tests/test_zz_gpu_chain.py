@@ -9,11 +9,7 @@ import copy
 import numpy as np
 import pytest
 
-# Reported, not gating: the frame-chain host paths were written when the round's GPU time was nearly spent and this file has
-# no recorded run on hardware (its host side is covered without a GPU by tests/test_host_pipeline_cpu.py and it was
-# pre-flighted against the host model, tools/preflight_gpu_tests.py).  A pass shows up as XPASS in the GPU tier's record,
-# a failure as xfail; the file is collected last so that nothing runs after it.
-pytestmark = [pytest.mark.gpu, pytest.mark.xfail(strict=False, reason="frame chains: no recorded run on a GPU yet")]
+pytestmark = pytest.mark.gpu
 
 FIELDS = ("T_cur_w", "n_tracked", "H", "seg_killed", "iters", "status", "patch_iters", "patch_levels")
 

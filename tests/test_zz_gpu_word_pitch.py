@@ -1,16 +1,14 @@
 """Lean level shipping for image widths whose finest shipped level is word aligned but not 16-byte aligned (752-pixel-wide
 cameras: level 2 has 188-byte rows).  The host layout of such a level is kept on the device, the pyramid kernel cannot read
 it (16-byte row loads), so the coarser levels are halfSampled by the alignment kernel itself, pair by pair — the code the
-arrival-gated stream uses, here on the plain and chunked host paths.  Collected after the other GPU files (this path was
-added without GPU time left in the round; tests/test_host_pipeline_cpu.py covers its host side)."""
+arrival-gated stream uses, here on the plain and chunked host paths (tests/test_host_pipeline_cpu.py covers its host side
+without a GPU)."""
 import copy
 
 import numpy as np
 import pytest
 
-# Reported, not gating: this path has never run on hardware (its host side and this file were pre-flighted against the host
-# model, tools/preflight_gpu_tests.py).  A pass shows up as XPASS in the GPU tier's record, a failure as xfail.
-pytestmark = [pytest.mark.gpu, pytest.mark.xfail(strict=False, reason="added after the round's GPU time was spent: not yet verified on a GPU")]
+pytestmark = pytest.mark.gpu
 
 FIELDS = ("T_cur_w", "n_tracked", "H", "seg_killed", "iters", "status", "patch_iters", "patch_levels")
 
