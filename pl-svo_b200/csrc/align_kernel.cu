@@ -86,6 +86,8 @@ struct PairCtl {
   double cand[7];  // candidate model T*exp(-x) of the current pass and its rotation matrix / step norm
   double candR[9];
   double cand_nm;
+  // the level's scale 2^-l and Jacobian factors focal/2^l and its square (:262), read by the pass loop at each use
+  double dscale, cJ, cJ2;
   float seg_chi2f; // seg_chi2 of the current pass (:683), summed by a third warp while the walker chains the points
   float chi2f;     // chi2 of the current pass, summed in the reference's order (walker warp -> thread 0)
   int n_opq;       // opaque patches of the current pass
@@ -138,7 +140,7 @@ __host__ __device__ inline Layout make_layout(int n_pts, int n_segs, int max_pat
   L.pt_vis = o;
   o += (uint32_t)n_pts;
   L.xyz = align_up(o, 16);
-  o = L.xyz + 3u * 8u * (uint32_t)max_patches;  // X/Z, Y/Z, 1/Z of every patch's 3-D point in the ref frame
+  o = L.xyz + 3u * 8u * (uint32_t)max_patches;  // X/Z, Y/Z, 1/Z of every patch's 3-D point in the ref frame, patch by patch
   L.tsc = o;
   o += 16u * 4u * (uint32_t)nt;  // the 16 chi2 terms of each thread's current patch ([k][tid]: conflict-free)
   o = align_up(o, 128);
@@ -247,16 +249,16 @@ __device__ __forceinline__ float row_px(uint32_t lo, uint32_t hi, int k) {
 // (R*xyz_ref + t) / Z_ref for the point (xn, yn, zi) = (X/Z, Y/Z, 1/Z), projected into the current image at this
 // level (world2cam(xyz)*scale, :425).  The pass's pose is read from shared memory here, at each use: held in registers
 // across the pass it would take 24 of the 128 registers of <128,4> and push the accumulators into local memory.
-__device__ __forceinline__ void project(const PairCtl* ctl, const AlignArgs& a, double dscale, double xn, double yn,
-                                        double zi, double& u, double& v) {
+__device__ __forceinline__ void project(const PairCtl* ctl, const AlignArgs& a, double xn, double yn, double zi, double& u,
+                                        double& v) {
   const double* R = ctl->R;
   const double* t = ctl->t;
   const double xc = R[0] * xn + R[1] * yn + (R[2] + t[0] * zi);
   const double yc = R[3] * xn + R[4] * yn + (R[5] + t[1] * zi);
   const double zc = R[6] * xn + R[7] * yn + (R[8] + t[2] * zi);
   const double izc = __drcp_rn(zc);
-  u = (a.fx * (xc * izc) + a.cx) * dscale;
-  v = (a.fy * (yc * izc) + a.cy) * dscale;
+  u = (a.fx * (xc * izc) + a.cx) * ctl->dscale;
+  v = (a.fy * (yc * izc) + a.cy) * ctl->dscale;
 }
 // seven consecutive bytes (reference image, global memory, read-only path)
 __device__ __forceinline__ void load_row7(const uint8_t* row, int sh, float* g) {
@@ -668,9 +670,9 @@ __global__ void __launch_bounds__(NT, MINB) sparse_img_align_kernel(const AlignA
         depth = sqrt(dx * dx + dy * dy + dz * dz);
       }
       const double zi = 1.0 / (f[2] * depth);  // z_inv of Frame::jacobian_xyz2uv (frame.h:144), constant per pair
-      xyz[0 * MP + i] = (f[0] * depth) * zi;
-      xyz[1 * MP + i] = (f[1] * depth) * zi;
-      xyz[2 * MP + i] = zi;
+      xyz[3 * i + 0] = (f[0] * depth) * zi;
+      xyz[3 * i + 1] = (f[1] * depth) * zi;
+      xyz[3 * i + 2] = zi;
     }
     for (int j = tid; j < ns; j += NT) {
       seg_alive[j] = a.seg_valid ? (a.seg_valid[so + j] ? 1 : 0) : 1;
@@ -700,6 +702,9 @@ __global__ void __launch_bounds__(NT, MINB) sparse_img_align_kernel(const AlignA
         }
         ctl->iter = 0;
         for (int i = 0; i < 7; ++i) ctl->old_model[i] = ctl->model[i];
+        ctl->dscale = dscale;
+        ctl->cJ = fabs(a.fx) / (double)(1 << level);  // focal_length / 2^level (:262)
+        ctl->cJ2 = ctl->cJ * ctl->cJ;
       }
       // ---- segment sampling at this level (:285-332) ----
       for (int j = tid; j < ns; j += NT) {
@@ -809,9 +814,9 @@ __global__ void __launch_bounds__(NT, MINB) sparse_img_align_kernel(const AlignA
             seg_px[2 * sp_idx] = px0;
             seg_px[2 * sp_idx + 1] = px1;
             const double zi = 1.0 / Z;
-            xyz[0 * MP + np + sp_idx] = X * zi;
-            xyz[1 * MP + np + sp_idx] = Y * zi;
-            xyz[2 * MP + np + sp_idx] = zi;
+            xyz[3 * (np + sp_idx) + 0] = X * zi;
+            xyz[3 * (np + sp_idx) + 1] = Y * zi;
+            xyz[3 * (np + sp_idx) + 2] = zi;
           }
           px0 += inc2d0, px1 += inc2d1;
           X += i0, Y += i1, Z += i2;
@@ -850,17 +855,15 @@ __global__ void __launch_bounds__(NT, MINB) sparse_img_align_kernel(const AlignA
       PHASE_MARK(kPhSetup);
 
       // ---- Gauss-Newton iterations at this level (vk::NLLSSolver::optimizeGaussNewton) ----
-      const double cJ = fabs(a.fx) / (double)(1 << level);  // focal_length / 2^level (:262)
-      const double cJ2 = cJ * cJ;
       for (;;) {
-        int n_meas_acc = 0, n_patch_acc = 0;
+        int n_pt_acc = 0;  // point patches evaluated: 16 measurements each
 #ifdef PLSVO_TREE_CHI2
         double chi2_tree = 0.0;
 #endif
         // this thread's 21 (upper-triangular H) + 6 (Jres) accumulators of the pass
-        double acc[32];
+        double acc[27];
 #pragma unroll
-        for (int i = 0; i < 32; ++i) acc[i] = 0.0;
+        for (int i = 0; i < 27; ++i) acc[i] = 0.0;
         double prefix_rounds = 0.0;  // estimate of the float chi2 accumulator after all earlier rounds
         // ======== point patches (:380-502), one round of NT consecutive patches at a time ========
         for (int r = 0; r < rounds; ++r) {
@@ -869,16 +872,17 @@ __global__ void __launch_bounds__(NT, MINB) sparse_img_align_kernel(const AlignA
           float Tf = 0.f;
           bool ok = false;
           if (p < np && pt_vis[p]) {
-            const double xn = xyz[0 * MP + p], yn = xyz[1 * MP + p], zi = xyz[2 * MP + p];
+            const double* X = xyz + 3 * p;
             double u, v;
-            project(ctl, a, dscale, xn, yn, zi, u, v);
+            project(ctl, a, X[0], X[1], X[2], u, v);
             double S[5];
             ok = eval_patch<true, NT>(cur_img, pitch, cols, rows, cache, MP, p, u, v, S, tsc, Tf);
             if (ok) {
-              // normal equations: rank-2 update with the two projection-Jacobian rows of the patch
-              rank2_update(acc, xn, yn, zi, S[0] * cJ2, S[1] * cJ2, S[2] * cJ2, S[3] * cJ, S[4] * cJ);
-              n_meas_acc += 16;
-              n_patch_acc += 1;
+              // normal equations: rank-2 update with the two projection-Jacobian rows of the patch.  The point and the
+              // level's factors are read again here rather than held across eval_patch, whose loop needs the registers.
+              const double cJ = ctl->cJ, cJ2 = ctl->cJ2;
+              rank2_update(acc, X[0], X[1], X[2], S[0] * cJ2, S[1] * cJ2, S[2] * cJ2, S[3] * cJ, S[4] * cJ);
+              n_pt_acc += 1;
             }
           }
           if (!ok) Tf = 0.f;  // not evaluated: contributes nothing (its scratch terms are stale and never read)
@@ -973,6 +977,7 @@ __global__ void __launch_bounds__(NT, MINB) sparse_img_align_kernel(const AlignA
 #endif
           PHASE_MARK(kPhPtChi2);
         }
+        int n_meas_acc = 16 * n_pt_acc, n_patch_acc = n_pt_acc;
         // ======== segment samples (:504-695).  Every segment owns a group of G = 2^k consecutive lanes of one warp
         // (G >= its sample count, or the whole warp looping over samples), so the per-segment gate / weight
         // (:640-688) is a few shuffles: no block barrier.  Warps take segment rounds from the top so they interleave
@@ -1008,7 +1013,7 @@ __global__ void __launch_bounds__(NT, MINB) sparse_img_align_kernel(const AlignA
             if (active) {
               p = np + off + n;
               double u, v;
-              project(ctl, a, dscale, xyz[0 * MP + p], xyz[1 * MP + p], xyz[2 * MP + p], u, v);
+              project(ctl, a, xyz[3 * p + 0], xyz[3 * p + 1], xyz[3 * p + 2], u, v);
               ok = eval_patch<false, NT>(cur_img, pitch, cols, rows, cache, MP, p, u, v, S, tsc, Tf);
               if (ok) {
                 ok_trips |= 1u << (trip & 31);
@@ -1049,8 +1054,8 @@ __global__ void __launch_bounds__(NT, MINB) sparse_img_align_kernel(const AlignA
             res_ = (float)((double)res_ / (double)(unsigned long long)N);  // :647
             if (good && (double)res_ < 200.0) {
               const float w = (float)(1.0 / (1.0 + (double)res_));  // :675
-              sH = (double)w / (double)res_ * cJ2;                  // H += H_*weight/res_ (:681)
-              sJ = (double)w * cJ;                                  // Jres += Jres_*weight (:682)
+              sH = (double)w / (double)res_ * ctl->cJ2;             // H += H_*weight/res_ (:681)
+              sJ = (double)w * ctl->cJ;                             // Jres += Jres_*weight (:682)
               seg_term[j] = __fmul_rn(__fmul_rn(res_, res_), w);    // chi2 += res_*res_*weight (:683)
 #ifdef PLSVO_TREE_CHI2
               chi2_tree += (double)seg_term[j];
@@ -1065,27 +1070,33 @@ __global__ void __launch_bounds__(NT, MINB) sparse_img_align_kernel(const AlignA
           sJ = __shfl_sync(0xffffffffu, sJ, gbase);
           if (sH != 0.0 || sJ != 0.0) {  // accepted segment: its samples enter the normal equations
             if (trips == 1) {
-              if (ok_trips) rank2_update(acc, xyz[0 * MP + p], xyz[1 * MP + p], xyz[2 * MP + p], S[0] * sH, S[1] * sH, S[2] * sH,
+              if (ok_trips) rank2_update(acc, xyz[3 * p + 0], xyz[3 * p + 1], xyz[3 * p + 2], S[0] * sH, S[1] * sH, S[2] * sH,
                                          S[3] * sJ, S[4] * sJ);
             } else {
               for (int trip = 0; trip < trips && trip < a.rec_cap; ++trip) {
                 if (!((ok_trips >> (trip & 31)) & 1u)) continue;
                 const int pp = np + off + n0 + trip * G;
                 const double* rp = rec + trip * NT + tid;
-                rank2_update(acc, xyz[0 * MP + pp], xyz[1 * MP + pp], xyz[2 * MP + pp], rp[0] * sH, rp[RS] * sH, rp[2 * RS] * sH,
+                rank2_update(acc, xyz[3 * pp + 0], xyz[3 * pp + 1], xyz[3 * pp + 2], rp[0] * sH, rp[RS] * sH, rp[2 * RS] * sH,
                              rp[3 * RS] * sJ, rp[4 * RS] * sJ);
               }
             }
           }
         }
         PHASE_MARK(kPhSeg);
-        acc[28] = (double)n_meas_acc;
-        acc[29] = (double)n_patch_acc;
+        // ---- block reduction (deterministic order) over the 32-slot layout of tot ----
+        double v[32];
+#pragma unroll
+        for (int i = 0; i < 27; ++i) v[i] = acc[i];
 #ifdef PLSVO_TREE_CHI2
-        acc[27] = chi2_tree;  // (variant for the A/B only) chi2 by tree sum, not in the reference's order
+        v[27] = chi2_tree;  // (variant for the A/B only) chi2 by tree sum, not in the reference's order
+#else
+        v[27] = 0.0;
 #endif
-        // ---- block reduction (deterministic order) ----
-        const double mine = warp_reduce32(acc, lane);
+        v[28] = (double)n_meas_acc;
+        v[29] = (double)n_patch_acc;
+        v[30] = 0.0, v[31] = 0.0;
+        const double mine = warp_reduce32(v, lane);
         red[warp * 32 + lane] = mine;
         __syncthreads();
         PHASE_MARK(kPhReduce);

@@ -449,19 +449,27 @@ __device__ __forceinline__ void bulk_g2s(void* dst_smem, const void* src_gmem, u
 
 __device__ __forceinline__ void fence_mbarrier_init() { asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); }
 
+// one butterfly step of warp_reduce32.  S is a template argument so that every index into v is a constant after
+// unrolling: a loop whose trip count depends on the step leaves v indexed at run time, and that puts v in local memory.
+template <int S>
+__device__ __forceinline__ void warp_reduce_step(double* v, int lane) {
+  const bool upper = (lane & S) != 0;
+#pragma unroll
+  for (int i = 0; i < S; ++i) {
+    const double send = upper ? v[i] : v[i + S];
+    const double keep = upper ? v[i + S] : v[i];
+    v[i] = keep + __shfl_xor_sync(0xffffffffu, send, S);
+  }
+}
+
 // register-halving warp reduction of 32 doubles: afterwards lane L holds the warp-wide sum of v[L]
 // (fixed summation order -> bitwise reproducible).
 __device__ __forceinline__ double warp_reduce32(double* v, int lane) {
-#pragma unroll
-  for (int s = 16; s >= 1; s >>= 1) {
-    const bool upper = (lane & s) != 0;
-#pragma unroll
-    for (int i = 0; i < s; ++i) {
-      const double send = upper ? v[i] : v[i + s];
-      const double keep = upper ? v[i + s] : v[i];
-      v[i] = keep + __shfl_xor_sync(0xffffffffu, send, s);
-    }
-  }
+  warp_reduce_step<16>(v, lane);
+  warp_reduce_step<8>(v, lane);
+  warp_reduce_step<4>(v, lane);
+  warp_reduce_step<2>(v, lane);
+  warp_reduce_step<1>(v, lane);
   return v[0];
 }
 
