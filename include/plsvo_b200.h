@@ -269,6 +269,36 @@ typedef struct plsvo_pyramid_result {
 int plsvo_pyramid_batch_run(plsvo_ctx* ctx, const plsvo_pyramid_batch* in, const plsvo_pyramid_result* out);
 
 /* ------------------------------------------------------------------------------------------
+ * Frame rectification: vk::PinholeCamera::undistortImage (rpg_vikit pinhole_camera.cpp), as app/run_pipeline.cpp
+ * calls it on every raw frame before FrameHandlerMono::addImage, for B frames, followed by createImgPyramid.
+ * The camera carries the distorted vk::PinholeCamera constructor arguments.  As there, fabs(d0) <= 1e-7 means no
+ * distortion (the frame is copied, whatever d1..d4 are); otherwise the map is cv::initUndistortRectifyMap of the
+ * float-rounded K and (k1,k2,p1,p2,k3) = (d0..d4), CV_16SC2, and each frame is cv::remap(raw, rect, map1, map2,
+ * INTER_LINEAR) with a constant border of 0 — bit-identical to OpenCV's fixed-point path.
+ * The map is built on the device once per camera and cached in the context; a call with another camera (or image
+ * size) rebuilds it.  Host in, host out, synchronous.  level[0] of the result is required and receives the
+ * rectified frame; levels 1..n_levels-1 are its half-sampled pyramid (as plsvo_pyramid_batch_run); n_levels <= 7.
+ * ---------------------------------------------------------------------------------------- */
+typedef struct plsvo_pinhole_camera {
+  int32_t width, height;
+  double fx, fy, cx, cy;
+  double d[5]; /* d0..d4 = k1, k2, p1, p2, k3 */
+} plsvo_pinhole_camera;
+
+typedef struct plsvo_undistort_batch {
+  plsvo_pinhole_camera cam;
+  int32_t batch, n_levels;
+  const uint8_t* img0; /* [B] raw frames of cam.width x cam.height: frame b at img0 + b*stride0, rows pitch0 bytes */
+  size_t pitch0, stride0;
+} plsvo_undistort_batch;
+
+int plsvo_undistort_batch_run(plsvo_ctx* ctx, const plsvo_undistort_batch* in, const plsvo_pyramid_result* out);
+
+/* device time (CUDA events) of the map build the last plsvo_undistort_batch_run call made, or -1 in *ms when that
+ * call reused the context's cached map or needed none (d0 = 0).  plsvo_last_kernel_ms never includes it. */
+int plsvo_last_map_build_ms(plsvo_ctx* ctx, float* ms);
+
+/* ------------------------------------------------------------------------------------------
  * Feature alignment (SURVEY.md §8f "next", rank 1): feature_alignment::align2D,
  * include/plsvo/feature_alignment.h:49-55, src/feature_alignment.cpp:160-290 (scalar path) — the 8x8
  * inverse-compositional refinement Matcher::findMatchDirect runs per feature (src/matcher.cpp:201).
@@ -494,7 +524,9 @@ int plsvo_line_seed_update_batch_run(plsvo_ctx* ctx, const plsvo_line_seed_batch
 
 /* device time (CUDA events on the context's stream) of the kernel launched by the last
  * plsvo_pyramid / align2d / align1d / match_direct / seed_update / structopt _batch_run call: the kernel alone,
- * without the host<->device copies those calls also make.  Measurement aid, no reference counterpart. */
+ * without the host<->device copies those calls also make.  For plsvo_undistort_batch_run it covers the remap and
+ * pyramid kernels; a map build that call made is not included (plsvo_last_map_build_ms reports it).  Measurement aid,
+ * no reference counterpart. */
 int plsvo_last_kernel_ms(plsvo_ctx* ctx, float* ms);
 
 /* number of kernels this context has launched since creation (bench "gpu_launches") */

@@ -149,6 +149,30 @@ class PyramidResult(C.Structure):
     _fields_ = [("level", _u8p * MAX_LEVELS), ("pitch", C.c_size_t * MAX_LEVELS), ("stride", C.c_size_t * MAX_LEVELS)]
 
 
+class PinholeCamera(C.Structure):
+    """plsvo_pinhole_camera: the distorted vk::PinholeCamera constructor arguments."""
+    _fields_ = [("width", C.c_int32), ("height", C.c_int32), ("fx", C.c_double), ("fy", C.c_double), ("cx", C.c_double),
+                ("cy", C.c_double), ("d", C.c_double * 5)]
+
+
+class UndistortBatch(C.Structure):
+    _fields_ = [("cam", PinholeCamera), ("batch", C.c_int32), ("n_levels", C.c_int32), ("img0", _u8p), ("pitch0", C.c_size_t),
+                ("stride0", C.c_size_t)]
+
+
+def pyramid_levels(B: int, H: int, W: int, n_levels: int):
+    """Contiguous u8 output levels [B, H>>l, W>>l] for l < n_levels and the plsvo_pyramid_result pointing at all of them."""
+    r = PyramidResult()
+    levels = []
+    for l in range(n_levels):
+        out = np.empty((B, H >> l, W >> l), np.uint8)
+        levels.append(out)
+        r.level[l] = out.ctypes.data_as(_u8p)
+        r.pitch[l] = out.strides[1]
+        r.stride[l] = out.strides[0]
+    return levels, r
+
+
 class Align2DBatch(C.Structure):
     _fields_ = [("n_features", C.c_int32), ("n_images", C.c_int32), ("width", C.c_int32), ("height", C.c_int32),
                 ("n_iter", C.c_int32), ("reserved", C.c_int32),
@@ -411,6 +435,8 @@ ABI_SYMBOLS = [
     ("plsvo_track_batch_run", C.c_int, [C.c_void_p, _P(AlignBatch), _P(AlignParams), _P(PoseOptBatch), _P(PoseOptParams),
                                         _P(AlignResult), _P(PoseOptResult)]),
     ("plsvo_pyramid_batch_run", C.c_int, [C.c_void_p, _P(PyramidBatch), _P(PyramidResult)]),
+    ("plsvo_undistort_batch_run", C.c_int, [C.c_void_p, _P(UndistortBatch), _P(PyramidResult)]),
+    ("plsvo_last_map_build_ms", C.c_int, [C.c_void_p, _P(C.c_float)]),
     ("plsvo_align2d_batch_run", C.c_int, [C.c_void_p, _P(Align2DBatch), _P(Align2DResult)]),
     ("plsvo_align1d_batch_run", C.c_int, [C.c_void_p, _P(Align1DBatch), _P(Align1DResult)]),
     ("plsvo_match_direct_batch_run", C.c_int, [C.c_void_p, _P(MatchBatch), _P(MatchResult)]),

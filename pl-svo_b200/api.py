@@ -53,6 +53,13 @@ class Context:
         self.check(self.lib.plsvo_last_kernel_ms(self.handle, C.byref(ms)), "plsvo_last_kernel_ms")
         return float(ms.value)
 
+    def last_map_build_ms(self) -> float | None:
+        """Device time of the map build made by the last PinholeCamera.undistortImage call on this context, or None when
+        that call reused the cached map or needed none (plsvo_last_map_build_ms)."""
+        ms = C.c_float(0)
+        self.check(self.lib.plsvo_last_map_build_ms(self.handle, C.byref(ms)), "plsvo_last_map_build_ms")
+        return None if ms.value < 0 else float(ms.value)
+
     def launch_count(self) -> int:
         return int(self.lib.plsvo_launch_count(self.handle))
 
@@ -183,6 +190,41 @@ def createImgPyramid(img_level_0, n_levels: int, ctx: Context | None = None):
         r.stride[l] = out.strides[0]
     ctx.check(ctx.lib.plsvo_pyramid_batch_run(ctx.handle, C.byref(b), C.byref(r)), "plsvo_pyramid_batch_run")
     return levels
+
+
+class PinholeCamera:
+    """vk::PinholeCamera(width, height, fx, fy, cx, cy, d0, d1, d2, d3, d4) (rpg_vikit pinhole_camera.cpp), for the one
+    call the pipeline makes on every raw frame, undistortImage (app/run_pipeline.cpp:409-414)."""
+
+    def __init__(self, width: int, height: int, fx: float, fy: float, cx: float, cy: float,
+                 d0: float = 0.0, d1: float = 0.0, d2: float = 0.0, d3: float = 0.0, d4: float = 0.0):
+        self.struct = abi.PinholeCamera(int(width), int(height), fx, fy, cx, cy, (C.c_double * 5)(d0, d1, d2, d3, d4))
+
+    @property
+    def width(self) -> int:
+        return self.struct.width
+
+    @property
+    def height(self) -> int:
+        return self.struct.height
+
+    def undistortImage(self, raw, n_levels: int = 1, ctx: Context | None = None):
+        """Batched undistortImage followed by frame_utils::createImgPyramid: u8 raw frames [B,H,W] (rows may be padded)
+        -> list of n_levels arrays [B, H>>l, W>>l], level 0 the rectified frames, bit-identical to cv::remap with the
+        camera's CV_16SC2 map.  The map is built on the device once per camera and context."""
+        import numpy as np
+
+        ctx = ctx or default_context()
+        raw = np.asarray(raw)
+        if raw.dtype != np.uint8 or raw.ndim != 3 or raw.strides[2] != 1:
+            raise PlsvoError("undistortImage: raw frames must be u8 [B,H,W] with unit column stride")
+        B, H, W = raw.shape
+        if (W, H) != (self.width, self.height):
+            raise PlsvoError(f"undistortImage: frames are {W}x{H}, the camera is {self.width}x{self.height}")
+        b = abi.UndistortBatch(self.struct, B, n_levels, raw.ctypes.data_as(C.POINTER(C.c_uint8)), raw.strides[1], raw.strides[0])
+        levels, r = abi.pyramid_levels(B, H, W, max(0, min(n_levels, abi.MAX_LEVELS)))
+        ctx.check(ctx.lib.plsvo_undistort_batch_run(ctx.handle, C.byref(b), C.byref(r)), "plsvo_undistort_batch_run")
+        return levels
 
 
 class feature_alignment:

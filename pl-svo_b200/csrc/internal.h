@@ -125,6 +125,33 @@ struct PyramidArgs {
 };
 cudaError_t pyramid_kernel_launch(const PyramidArgs& a, cudaStream_t s);
 
+// ---------------------------------------------------------------------------------------------
+// vk::PinholeCamera::undistortImage: the CV_16SC2 map of cv::initUndistortRectifyMap, then cv::remap INTER_LINEAR.
+// The two launchers are weak references: plsvo_abi.cu is also compiled, unchanged, into the host-pipeline model of the
+// tests, whose model kernels need not provide them; plsvo_undistort_batch_run then reports them missing.  The library
+// always links undistort_kernel.cu.
+constexpr int kRemapTileW = 64;  // map rows are padded to a multiple of this (whole tiles load without bounds checks)
+struct UndistortMapArgs {
+  int width, height, map_pitch;                 // map_pitch: entries per map row
+  double fx, fy, cx, cy, k1, k2, p1, p2, k3;    // already rounded to float (vikit's Mat_<float> cvK_ / cvD_)
+  short2* map1;                                 // [height][map_pitch] (x, y) source pixel
+  uint16_t* map2;                               // [height][map_pitch] (iv & 31) * 32 + (iu & 31)
+};
+__attribute__((weak)) cudaError_t undistort_map_launch(const UndistortMapArgs& a, cudaStream_t s);
+
+struct RemapArgs {
+  int B, width, height, map_pitch;
+  const short2* map1;
+  const uint16_t* map2;
+  const uint8_t* src;  // [B][height][src_pitch] raw frames (src_pitch multiple of 16)
+  uint32_t src_pitch;
+  size_t src_stride;
+  uint8_t* dst;        // [B][height][dst_pitch] rectified frames: pyramid level 0 (dst_pitch multiple of 16)
+  uint32_t dst_pitch;
+  size_t dst_stride;
+};
+__attribute__((weak)) cudaError_t undistort_remap_launch(const RemapArgs& a, int num_sms, cudaStream_t s);
+
 
 // ---------------------------------------------------------------------------------------------
 struct Align2DArgs {

@@ -83,6 +83,13 @@ struct plsvo_ctx_impl {
       m_olvl, m_oA;  // findMatchDirect
   DevBuf d_sa, d_sb, d_smu, d_szr, d_ssig, d_smu_e, d_szr_e, d_ssig_e, d_sout;  // depth-filter seeds
   DevBuf s_T, s_pb, s_pf, s_pof, s_pp, s_sb, s_sf, s_ssf, s_sef, s_sp, s_ep, s_out;  // structure optimisation
+  // undistortion: raw frames, and the map of the camera in u_cam (valid when u_map_ok), built on the device
+  DevBuf u_raw, u_map1, u_map2;
+  plsvo_pinhole_camera u_cam;
+  int u_map_pitch = 0;
+  bool u_map_ok = false;
+  bool u_map_built = false;  // the last undistort call built the map (timed by u_map_ev)
+  cudaEvent_t u_map_ev[2] = {nullptr, nullptr};
   DevBuf p_out_T, p_out_cov, p_out_scale, p_out_ei, p_out_ef, p_out_npt, p_out_nls, p_out_pto, p_out_sgo, p_out_iters,
       p_out_status;
 };
@@ -108,14 +115,17 @@ int fail(plsvo_ctx_impl* c, int code, const char* what, cudaError_t e = cudaSucc
     if (e_ != cudaSuccess) return fail(c, PLSVO_ERR_CUDA, #call, e_);   \
   } while (0)
 
-// Records one of the two timing events around the kernel of a host-in/host-out entry point.
-cudaError_t kernel_timer(plsvo_ctx_impl* c, int which, cudaStream_t s) {
-  if (!c->k_ev[which]) {
-    cudaError_t e = cudaEventCreate(&c->k_ev[which]);
+// Records a timing event, creating it on first use.
+cudaError_t record_event(cudaEvent_t& ev, cudaStream_t s) {
+  if (!ev) {
+    cudaError_t e = cudaEventCreate(&ev);
     if (e != cudaSuccess) return e;
   }
-  return cudaEventRecord(c->k_ev[which], s);
+  return cudaEventRecord(ev, s);
 }
+
+// Records one of the two timing events around the kernel of a host-in/host-out entry point.
+cudaError_t kernel_timer(plsvo_ctx_impl* c, int which, cudaStream_t s) { return record_event(c->k_ev[which], s); }
 
 cudaError_t ensure(DevBuf& b, size_t bytes) {
   if (bytes <= b.cap && b.p) return cudaSuccess;
@@ -233,7 +243,8 @@ void plsvo_ctx_destroy(plsvo_ctx* ctx) {
                     &c->p_pt_count,  &c->p_pt_f,     &c->p_pt_pos,    &c->p_pt_level,   &c->p_pt_valid,  &c->p_seg_count,
                     &c->p_seg_line,  &c->p_seg_spos, &c->p_seg_epos,  &c->p_seg_level,  &c->p_seg_valid, &c->p_out_T,
                     &c->p_out_cov,   &c->p_out_scale, &c->p_out_ei,   &c->p_out_ef,     &c->p_out_npt,   &c->p_out_nls,
-                    &c->p_out_pto,   &c->p_out_sgo,  &c->p_out_iters, &c->p_out_status};
+                    &c->p_out_pto,   &c->p_out_sgo,  &c->p_out_iters, &c->p_out_status, &c->u_raw,      &c->u_map1,
+                    &c->u_map2};
   for (DevBuf* b : bufs) release(*b);
   if (c->h_flags) cudaFreeHost(c->h_flags);
   if (c->h_out) cudaFreeHost(c->h_out);
@@ -250,6 +261,8 @@ void plsvo_ctx_destroy(plsvo_ctx* ctx) {
     if (c->chunk_ev[k]) cudaEventDestroy(c->chunk_ev[k]);
   if (c->start_ev) cudaEventDestroy(c->start_ev);
   for (auto& e : c->k_ev)
+    if (e) cudaEventDestroy(e);
+  for (auto& e : c->u_map_ev)
     if (e) cudaEventDestroy(e);
   if (c->own_stream) cudaStreamDestroy(c->stream);
   delete c;
@@ -1809,6 +1822,125 @@ extern "C" int plsvo_line_seed_update_batch_run(plsvo_ctx* ctx, const plsvo_line
 extern "C" int plsvo_pyramid_batch_run(plsvo_ctx* ctx, const plsvo_pyramid_batch* in, const plsvo_pyramid_result* out) {
   if (!ctx || !in || !out) return PLSVO_ERR_INVALID;
   return settled(CTX(ctx), pyramid_batch_run_body(ctx, in, out));
+}
+
+// vk::PinholeCamera::undistortImage + createImgPyramid for B frames: raw frames up, map (built once per camera), remap
+// into level 0, pyramid kernel for levels 1.., every level down.
+static int undistort_batch_run_body(plsvo_ctx* ctx, const plsvo_undistort_batch* in, const plsvo_pyramid_result* out) {
+  plsvo_ctx_impl* c = CTX(ctx);
+  c->u_map_built = false;
+  const plsvo_pinhole_camera& cam = in->cam;
+  const int W = cam.width, H = cam.height;
+  if (in->batch <= 0 || W <= 0 || H <= 0) return fail(c, PLSVO_ERR_INVALID, "undistort batch: batch, width and height must be positive");
+  if (in->n_levels < 1 || in->n_levels > 7) return fail(c, PLSVO_ERR_INVALID, "undistort batch: n_levels must be in [1,7]");
+  if (!in->img0) return fail(c, PLSVO_ERR_INVALID, "undistort batch: raw frames missing (img0 is NULL)");
+  if (in->pitch0 < (size_t)W) return fail(c, PLSVO_ERR_INVALID, "undistort batch: pitch0 smaller than the image width");
+  // vikit hands the parameters to OpenCV as Mat_<float>: they must stay finite, and fx, fy non-zero, after that rounding
+  const double par[9] = {cam.fx, cam.fy, cam.cx, cam.cy, cam.d[0], cam.d[1], cam.d[2], cam.d[3], cam.d[4]};
+  for (double p : par)
+    if (!isfinite(p) || !isfinite((float)p)) return fail(c, PLSVO_ERR_INVALID, "undistort camera: a parameter is not finite in float");
+  if ((float)cam.fx == 0.f || (float)cam.fy == 0.f) return fail(c, PLSVO_ERR_INVALID, "undistort camera: fx and fy must be non-zero");
+  for (int l = 0; l < in->n_levels; ++l) {
+    const int cols = W >> l, rows = H >> l;
+    if (cols <= 0 || rows <= 0) return fail(c, PLSVO_ERR_INVALID, "pyramid level smaller than one pixel");
+    if (!out->level[l]) return fail(c, PLSVO_ERR_INVALID, "output level missing (level 0 receives the rectified frame)");
+    if (out->pitch[l] < (size_t)cols) return fail(c, PLSVO_ERR_INVALID, "output pitch smaller than the level width");
+  }
+  // PinholeCamera's distortion_ flag: without it undistortImage is a copy, so the raw frames go straight to level 0
+  const bool distortion = fabs(cam.d[0]) > 0.0000001;
+  if (distortion && (!undistort_map_launch || !undistort_remap_launch))
+    return fail(c, PLSVO_ERR_CUDA, "undistort kernels are not linked into this library", cudaErrorNotSupported);
+  CK(cudaSetDevice(c->device));
+  PyramidArgs a;
+  memset(&a, 0, sizeof a);
+  a.B = in->batch, a.width = W, a.height = H, a.n_levels = in->n_levels;
+  const size_t B = (size_t)in->batch;
+  size_t total = 0, off[PLSVO_MAX_LEVELS] = {0};
+  for (int l = 0; l < in->n_levels; ++l) {
+    a.pitch[l] = (uint32_t)(((W >> l) + 15) / 16 * 16);
+    a.stride[l] = (size_t)(H >> l) * a.pitch[l];
+    total = (total + 255) / 256 * 256;
+    off[l] = total;
+    total += a.stride[l] * B;
+  }
+  CK(ensure(c->y_img, total + 256));
+  for (int l = 0; l < in->n_levels; ++l) a.level[l] = static_cast<uint8_t*>(c->y_img.p) + off[l];
+  cudaStream_t s = c->stream;
+  uint8_t* raw = a.level[0];
+  if (distortion) {
+    CK(ensure(c->u_raw, a.stride[0] * B));
+    raw = static_cast<uint8_t*>(c->u_raw.p);
+  }
+  if (in->stride0 == (size_t)H * in->pitch0) {
+    CK(cudaMemcpy2DAsync(raw, a.pitch[0], in->img0, in->pitch0, W, (size_t)H * B, cudaMemcpyHostToDevice, s));
+  } else {
+    for (size_t b = 0; b < B; ++b)
+      CK(cudaMemcpy2DAsync(raw + b * a.stride[0], a.pitch[0], in->img0 + b * in->stride0, in->pitch0, W, H, cudaMemcpyHostToDevice, s));
+  }
+  if (distortion && (!c->u_map_ok || memcmp(&c->u_cam, &cam, sizeof cam) != 0)) {
+    c->u_map_ok = false;
+    const int mp = (W + kRemapTileW - 1) / kRemapTileW * kRemapTileW;
+    const size_t n = (size_t)H * mp;
+    CK(ensure(c->u_map1, n * sizeof(short2)));
+    CK(ensure(c->u_map2, n * sizeof(uint16_t)));
+    CK(cudaMemsetAsync(c->u_map1.p, 0, n * sizeof(short2), s));  // the row padding: read by whole-tile loads, never used
+    CK(cudaMemsetAsync(c->u_map2.p, 0, n * sizeof(uint16_t), s));
+    UndistortMapArgs m;
+    m.width = W, m.height = H, m.map_pitch = mp;
+    m.fx = (float)cam.fx, m.fy = (float)cam.fy, m.cx = (float)cam.cx, m.cy = (float)cam.cy;
+    m.k1 = (float)cam.d[0], m.k2 = (float)cam.d[1], m.p1 = (float)cam.d[2], m.p2 = (float)cam.d[3], m.k3 = (float)cam.d[4];
+    m.map1 = static_cast<short2*>(c->u_map1.p);
+    m.map2 = static_cast<uint16_t*>(c->u_map2.p);
+    CK(record_event(c->u_map_ev[0], s));
+    CK(undistort_map_launch(m, s));
+    CK(record_event(c->u_map_ev[1], s));
+    c->launches += 1;
+    c->u_cam = cam, c->u_map_pitch = mp, c->u_map_ok = true, c->u_map_built = true;
+  }
+  CK(kernel_timer(c, 0, s));
+  if (distortion) {
+    RemapArgs r;
+    r.B = in->batch, r.width = W, r.height = H, r.map_pitch = c->u_map_pitch;
+    r.map1 = static_cast<const short2*>(c->u_map1.p), r.map2 = static_cast<const uint16_t*>(c->u_map2.p);
+    r.src = raw, r.src_pitch = a.pitch[0], r.src_stride = a.stride[0];
+    r.dst = a.level[0], r.dst_pitch = a.pitch[0], r.dst_stride = a.stride[0];
+    CK(undistort_remap_launch(r, c->num_sms, s));
+    c->launches += 1;
+  }
+  if (in->n_levels > 1) {
+    CK(pyramid_kernel_launch(a, s));
+    c->launches += 1;
+  }
+  CK(kernel_timer(c, 1, s));
+  for (int l = 0; l < in->n_levels; ++l) {
+    const int cols = W >> l, rows = H >> l;
+    if (out->stride[l] == (size_t)rows * out->pitch[l]) {
+      CK(cudaMemcpy2DAsync(out->level[l], out->pitch[l], a.level[l], a.pitch[l], cols, (size_t)rows * B, cudaMemcpyDeviceToHost, s));
+    } else {
+      for (size_t b = 0; b < B; ++b)
+        CK(cudaMemcpy2DAsync(out->level[l] + b * out->stride[l], out->pitch[l], a.level[l] + b * a.stride[l], a.pitch[l], cols, rows,
+                             cudaMemcpyDeviceToHost, s));
+    }
+  }
+  CK(cudaStreamSynchronize(s));
+  return PLSVO_OK;
+}
+
+extern "C" int plsvo_undistort_batch_run(plsvo_ctx* ctx, const plsvo_undistort_batch* in, const plsvo_pyramid_result* out) {
+  if (!ctx || !in || !out) return PLSVO_ERR_INVALID;
+  return settled(CTX(ctx), undistort_batch_run_body(ctx, in, out));
+}
+
+extern "C" int plsvo_last_map_build_ms(plsvo_ctx* ctx, float* ms) {
+  if (!ctx || !ms) return PLSVO_ERR_INVALID;
+  plsvo_ctx_impl* c = CTX(ctx);
+  if (!c->u_map_built) {
+    *ms = -1.f;
+    return PLSVO_OK;
+  }
+  CK(cudaEventSynchronize(c->u_map_ev[1]));
+  CK(cudaEventElapsedTime(ms, c->u_map_ev[0], c->u_map_ev[1]));
+  return PLSVO_OK;
 }
 
 extern "C" int plsvo_match_direct_batch_run(plsvo_ctx* ctx, const plsvo_match_batch* in, const plsvo_match_result* out) {
