@@ -299,6 +299,46 @@ int plsvo_undistort_batch_run(plsvo_ctx* ctx, const plsvo_undistort_batch* in, c
 int plsvo_last_map_build_ms(plsvo_ctx* ctx, float* ms);
 
 /* ------------------------------------------------------------------------------------------
+ * Alignment and tracking of raw frames: plsvo_undistort_batch_run followed by plsvo_align_batch_run /
+ * plsvo_track_batch_run in one call, without the rectified pyramid leaving the device.  One kernel rectifies each frame
+ * (the context's cached map, as plsvo_undistort_batch_run) and half-samples it, and stores only the levels alignment
+ * reads plus those asked for in rect_out.  Results are byte-identical to the two calls chained through the host, with
+ * plsvo_align_batch_run / plsvo_track_batch_run on their plain upload -> launch -> download sequence (the one they take
+ * below 256 pairs; the arrival-gated path they take for larger batches uses another CTA shape and agrees to round-off).
+ * The raw calls always take the plain sequence.
+ *
+ * - `batch` describes features, poses and the UNDISTORTED camera exactly as for plsvo_align_batch_run; every
+ *   ref_img[l] / cur_img[l] must be NULL (the images come from `raw`).  batch->cam must equal raw->cam in width, height,
+ *   fx, fy, cx and cy (run_pipeline builds both cameras from the same values).  flags = PLSVO_ALIGN_FRAME_CHAIN takes
+ *   B+1 raw frames in ref_raw, pair b = (frame b, frame b+1), and cur_raw must be NULL.
+ * - fabs(raw->cam.d[0]) <= 1e-7 means no distortion: the raw frame is level 0 as it is.
+ * - max_level <= 6 (one 64x64 level-0 tile per CTA holds levels 0..6).
+ * - rect_out may be NULL.  Each non-NULL rect_out->level[l] (l <= 6) receives rectified level l of every frame in stack
+ *   order: the B+1 frames of a chain, or the B reference frames followed by the B current frames.  Levels left NULL are
+ *   not copied back, and not written at all unless alignment reads them.
+ * - Malformed input (K mismatch, image pointers in `batch`, a NULL raw stack, cur_raw with a chain, pitch < width,
+ *   non-finite parameters or zero fx / fy after rounding to float, max_level > 6, a rect_out level too narrow or smaller
+ *   than one pixel) returns PLSVO_ERR_INVALID with a message.  As every one-call form, these have finished with the
+ *   caller's arrays when they return, whatever they return.
+ * - plsvo_last_kernel_ms covers the rectify + pyramid kernel and the alignment (and pose-optimiser) kernels;
+ *   plsvo_last_map_build_ms reports a map build this call made.
+ * ---------------------------------------------------------------------------------------- */
+typedef struct plsvo_raw_frames {
+  plsvo_pinhole_camera cam; /* the distorted camera; d0..d4 as for plsvo_undistort_batch */
+  const uint8_t* ref_raw;   /* [B] raw frames of cam.width x cam.height, or [B+1] with PLSVO_ALIGN_FRAME_CHAIN */
+  const uint8_t* cur_raw;   /* [B] raw frames; must be NULL with PLSVO_ALIGN_FRAME_CHAIN */
+  size_t pitch, stride;     /* host layout of both stacks: frame k at ref_raw + k*stride, rows pitch bytes */
+} plsvo_raw_frames;
+
+int plsvo_align_raw_batch_run(plsvo_ctx* ctx, const plsvo_raw_frames* raw, const plsvo_align_batch* batch,
+                              const plsvo_align_params* params, const plsvo_align_result* out,
+                              const plsvo_pyramid_result* rect_out);
+int plsvo_track_raw_batch_run(plsvo_ctx* ctx, const plsvo_raw_frames* raw, const plsvo_align_batch* al_batch,
+                              const plsvo_align_params* al_params, const plsvo_poseopt_batch* po_batch,
+                              const plsvo_poseopt_params* po_params, const plsvo_align_result* al_out,
+                              const plsvo_poseopt_result* po_out, const plsvo_pyramid_result* rect_out);
+
+/* ------------------------------------------------------------------------------------------
  * Feature alignment (SURVEY.md §8f "next", rank 1): feature_alignment::align2D,
  * include/plsvo/feature_alignment.h:49-55, src/feature_alignment.cpp:160-290 (scalar path) — the 8x8
  * inverse-compositional refinement Matcher::findMatchDirect runs per feature (src/matcher.cpp:201).
@@ -525,7 +565,8 @@ int plsvo_line_seed_update_batch_run(plsvo_ctx* ctx, const plsvo_line_seed_batch
 /* device time (CUDA events on the context's stream) of the kernel launched by the last
  * plsvo_pyramid / align2d / align1d / match_direct / seed_update / structopt _batch_run call: the kernel alone,
  * without the host<->device copies those calls also make.  For plsvo_undistort_batch_run it covers the remap and
- * pyramid kernels; a map build that call made is not included (plsvo_last_map_build_ms reports it).  Measurement aid,
+ * pyramid kernels; a map build that call made is not included (plsvo_last_map_build_ms reports it).  For the raw-frame
+ * calls it covers the rectify + pyramid kernel and the alignment (and pose-optimiser) kernels.  Measurement aid,
  * no reference counterpart. */
 int plsvo_last_kernel_ms(plsvo_ctx* ctx, float* ms);
 

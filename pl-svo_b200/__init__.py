@@ -5,6 +5,6 @@ the `plsvo_b200` shim module at the repo root.
 """
 from . import abi, dist, synth  # noqa: F401
 from .api import (Context, DepthFilter, Matcher, PinholeCamera, SparseImgAlign, createImgPyramid, default_context, feature_alignment,  # noqa: F401
-                  optimizeStructure, pose_optimizer)
+                  optimizeStructure, pose_optimizer, track_raw)
 
 __version__ = "0.1.0"

@@ -160,6 +160,31 @@ class UndistortBatch(C.Structure):
                 ("stride0", C.c_size_t)]
 
 
+class RawFrames(C.Structure):
+    """plsvo_raw_frames: the distorted camera and the raw frame stacks of plsvo_align_raw_batch_run /
+    plsvo_track_raw_batch_run."""
+    _fields_ = [("cam", PinholeCamera), ("ref_raw", _u8p), ("cur_raw", _u8p), ("pitch", C.c_size_t), ("stride", C.c_size_t)]
+
+
+def make_raw_frames(cam: PinholeCamera, raw, batch: int):
+    """plsvo_raw_frames for `batch` pairs from raw u8 frames: one array [B+1,H,W] (a frame chain) or a pair (ref, cur) of
+    [B,H,W] arrays with the same strides.  Rows may be padded.  Returns (struct, chain, keepalive)."""
+    chain = not isinstance(raw, (tuple, list))
+    stacks = [np.asarray(raw)] if chain else [np.asarray(x) for x in raw]
+    if not chain and len(stacks) != 2:
+        raise ValueError("raw frames: one [B+1,H,W] chain or a (ref, cur) pair of [B,H,W] stacks")
+    for s in stacks:
+        if s.dtype != np.uint8 or s.ndim != 3 or s.strides[2] != 1 or s.shape[1:] != (cam.height, cam.width):
+            raise ValueError(f"raw frames must be u8 [n,{cam.height},{cam.width}] with unit column stride")
+        if s.shape[0] != batch + (1 if chain else 0):
+            raise ValueError(f"raw frames: {s.shape[0]} frames for {batch} pairs" + (" (a chain has B+1)" if chain else ""))
+        if s.strides != stacks[0].strides:
+            raise ValueError("raw frames: both stacks must have the same layout")
+    r = RawFrames(cam, stacks[0].ctypes.data_as(_u8p), None if chain else stacks[1].ctypes.data_as(_u8p),
+                  stacks[0].strides[1], stacks[0].strides[0])
+    return r, chain, stacks
+
+
 def pyramid_levels(B: int, H: int, W: int, n_levels: int):
     """Contiguous u8 output levels [B, H>>l, W>>l] for l < n_levels and the plsvo_pyramid_result pointing at all of them."""
     r = PyramidResult()
@@ -437,6 +462,10 @@ ABI_SYMBOLS = [
     ("plsvo_pyramid_batch_run", C.c_int, [C.c_void_p, _P(PyramidBatch), _P(PyramidResult)]),
     ("plsvo_undistort_batch_run", C.c_int, [C.c_void_p, _P(UndistortBatch), _P(PyramidResult)]),
     ("plsvo_last_map_build_ms", C.c_int, [C.c_void_p, _P(C.c_float)]),
+    ("plsvo_align_raw_batch_run", C.c_int, [C.c_void_p, _P(RawFrames), _P(AlignBatch), _P(AlignParams), _P(AlignResult),
+                                            _P(PyramidResult)]),
+    ("plsvo_track_raw_batch_run", C.c_int, [C.c_void_p, _P(RawFrames), _P(AlignBatch), _P(AlignParams), _P(PoseOptBatch),
+                                            _P(PoseOptParams), _P(AlignResult), _P(PoseOptResult), _P(PyramidResult)]),
     ("plsvo_align2d_batch_run", C.c_int, [C.c_void_p, _P(Align2DBatch), _P(Align2DResult)]),
     ("plsvo_align1d_batch_run", C.c_int, [C.c_void_p, _P(Align1DBatch), _P(Align1DResult)]),
     ("plsvo_match_direct_batch_run", C.c_int, [C.c_void_p, _P(MatchBatch), _P(MatchResult)]),

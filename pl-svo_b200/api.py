@@ -126,6 +126,22 @@ class SparseImgAlign:
         self.last = out
         return out
 
+    def run_raw(self, camera: "PinholeCamera", raw, data, rect_levels=None):
+        """run() on raw (distorted) frames: each frame is rectified with `camera` (PinholeCamera.undistortImage) and
+        half-sampled on the device, and the pyramid never leaves it.  raw: a [B+1,H,W] frame chain, or a (ref, cur) pair
+        of [B,H,W] stacks; rows may be padded.  data describes features, poses and the undistorted camera as for run()
+        (its images are ignored).  Results are byte-identical to undistortImage followed by the plain host-buffer run().
+        rect_levels: levels to bring back as well; returns (AlignOut, {level: [n_frames, H>>l, W>>l]}) then, the frames
+        in stack order (the chain, or the reference frames followed by the current ones)."""
+        rf, batch, keep = _raw_call_args(camera, raw, data)
+        levels, r = _rect_outputs(camera, rf, data.batch, rect_levels)
+        out = abi.AlignOut(data.batch, data.n_segs)
+        self.ctx.check(self.ctx.lib.plsvo_align_raw_batch_run(self.ctx.handle, C.byref(rf), C.byref(batch), C.byref(self.params),
+                                                              C.byref(out.struct), C.byref(r) if r is not None else None),
+                       "plsvo_align_raw_batch_run")
+        self.last = out
+        return out if rect_levels is None else (out, levels)
+
     def getFisherInformation(self):
         """H_ / (5e-4 * 255^2), sparse_img_align.cpp:97-102 (per pair)."""
         if self.last is None:
@@ -169,6 +185,55 @@ def track(align_data, poseopt_data, max_level: int = 4, min_level: int = 2, n_it
     ctx.check(ctx.lib.plsvo_track_batch_run(ctx.handle, C.byref(ab), C.byref(ap), C.byref(pb), C.byref(pp), C.byref(ao.struct),
                                             C.byref(po.struct)), "plsvo_track_batch_run")
     return ao, po
+
+
+def _raw_call_args(camera, raw, align_data):
+    """plsvo_raw_frames and an image-free plsvo_align_batch (flags from the layout of `raw`) for the raw-frame calls."""
+    rf, chain, keep_r = abi.make_raw_frames(camera.struct, raw, align_data.batch)
+    batch, keep_a = abi.make_align_batch(align_data)
+    for l in range(abi.MAX_LEVELS):
+        batch.ref_img[l] = batch.cur_img[l] = None
+        batch.img_pitch[l] = batch.img_stride[l] = 0
+    batch.flags = abi.ALIGN_FRAME_CHAIN if chain else 0
+    return rf, batch, (keep_r, keep_a)
+
+
+def _rect_outputs(camera, rf, B: int, rect_levels):
+    """Host arrays for the rectified levels a raw-frame call brings back, and the plsvo_pyramid_result (or None)."""
+    import numpy as np
+
+    if rect_levels is None:
+        return None, None
+    n = B + 1 if not rf.cur_raw else 2 * B
+    r = abi.PyramidResult()
+    levels = {}
+    for l in rect_levels:
+        out = np.empty((n, camera.height >> l, camera.width >> l), np.uint8)
+        levels[l] = out
+        r.level[l] = out.ctypes.data_as(C.POINTER(C.c_uint8))
+        r.pitch[l], r.stride[l] = out.strides[1], out.strides[0]
+    return levels, r
+
+
+def track_raw(camera, raw, align_data, poseopt_data, max_level: int = 4, min_level: int = 2, n_iter: int = 30,
+              reproj_thresh: float = 2.0, po_n_iter: int = 10, po_n_iter_ref: int | None = None, chained: bool = True,
+              ctx: Context | None = None, rect_levels=None):
+    """track() on raw (distorted) frames, rectified with `camera` on the device (see SparseImgAlign.run_raw for `raw` and
+    `rect_levels`).  Returns (AlignOut, PoseOptOut), plus the dict of rectified levels when rect_levels is given."""
+    ctx = ctx or default_context()
+    ap = abi.align_params(max_level, min_level, n_iter)
+    pp = abi.poseopt_params(reproj_thresh, po_n_iter, -1 if po_n_iter_ref is None else po_n_iter_ref)
+    rf, ab, keep_a = _raw_call_args(camera, raw, align_data)
+    pb, keep_p = abi.make_poseopt_batch(poseopt_data)
+    if chained:
+        pb.T_f_w = abi._f64p()
+    levels, r = _rect_outputs(camera, rf, align_data.batch, rect_levels)
+    ao = abi.AlignOut(align_data.batch, align_data.n_segs)
+    po = abi.PoseOptOut(poseopt_data.batch, poseopt_data.n_pts, poseopt_data.n_segs)
+    ctx.check(ctx.lib.plsvo_track_raw_batch_run(ctx.handle, C.byref(rf), C.byref(ab), C.byref(ap), C.byref(pb), C.byref(pp),
+                                                C.byref(ao.struct), C.byref(po.struct), C.byref(r) if r is not None else None),
+              "plsvo_track_raw_batch_run")
+    return (ao, po) if rect_levels is None else (ao, po, levels)
 
 
 def createImgPyramid(img_level_0, n_levels: int, ctx: Context | None = None):

@@ -9,7 +9,7 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(_HERE, "csrc")
 SOURCES = ["align_kernel.cu", "poseopt_kernel.cu", "pyramid_kernel.cu", "align2d_kernel.cu", "structopt_kernel.cu", "undistort_kernel.cu",
            "plsvo_abi.cu"]
-HEADERS = ["device_math.cuh", "exact_math.cuh", "internal.h", os.path.join("..", "..", "include", "plsvo_b200.h")]
+HEADERS = ["device_math.cuh", "exact_math.cuh", "halfsample.cuh", "internal.h", os.path.join("..", "..", "include", "plsvo_b200.h")]
 OUT = os.path.join(CSRC, "libplsvo_b200.so")
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a",

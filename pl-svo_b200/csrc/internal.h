@@ -152,6 +152,22 @@ struct RemapArgs {
 };
 __attribute__((weak)) cudaError_t undistort_remap_launch(const RemapArgs& a, int num_sms, cudaStream_t s);
 
+// Rectification and half-sampling in one kernel (the raw-frame alignment calls): each CTA forms a 64x64 tile of
+// rectified level 0 from the raw frame with the remap arithmetic above (or copies it when map1 is NULL: no distortion),
+// half-samples it down to n_levels - 1, and stores only the levels whose level[l] is non-NULL.  Weak for the same reason
+// as the two launchers above.
+struct RawPyramidArgs {
+  int B, width, height, n_levels, map_pitch;       // n_levels <= 7
+  const short2* map1;                              // NULL: copy the raw frame (fabs(d0) <= 1e-7)
+  const uint16_t* map2;
+  const uint8_t* src;                              // [B][height][src_pitch] raw frames
+  size_t src_pitch, src_stride;
+  uint8_t* level[PLSVO_MAX_LEVELS];                // [B][rows_l][pitch_l], or NULL: level not stored
+  uint32_t pitch[PLSVO_MAX_LEVELS];                // multiples of 16
+  size_t stride[PLSVO_MAX_LEVELS];
+};
+__attribute__((weak)) cudaError_t undistort_pyramid_launch(const RawPyramidArgs& a, int num_sms, cudaStream_t s);
+
 
 // ---------------------------------------------------------------------------------------------
 struct Align2DArgs {

@@ -1824,6 +1824,43 @@ extern "C" int plsvo_pyramid_batch_run(plsvo_ctx* ctx, const plsvo_pyramid_batch
   return settled(CTX(ctx), pyramid_batch_run_body(ctx, in, out));
 }
 
+namespace {
+// The CV_16SC2 map of a distorted camera, built on the device when the context's cached map is of another camera (or
+// image size).  Sets u_map_built when it builds one (plsvo_last_map_build_ms).
+int undistort_map_ensure(plsvo_ctx_impl* c, const plsvo_pinhole_camera& cam, cudaStream_t s) {
+  if (c->u_map_ok && memcmp(&c->u_cam, &cam, sizeof cam) == 0) return PLSVO_OK;
+  const int W = cam.width, H = cam.height;
+  c->u_map_ok = false;
+  const int mp = (W + kRemapTileW - 1) / kRemapTileW * kRemapTileW;
+  const size_t n = (size_t)H * mp;
+  CK(ensure(c->u_map1, n * sizeof(short2)));
+  CK(ensure(c->u_map2, n * sizeof(uint16_t)));
+  CK(cudaMemsetAsync(c->u_map1.p, 0, n * sizeof(short2), s));  // the row padding: read by whole-tile loads, never used
+  CK(cudaMemsetAsync(c->u_map2.p, 0, n * sizeof(uint16_t), s));
+  UndistortMapArgs m;
+  m.width = W, m.height = H, m.map_pitch = mp;
+  m.fx = (float)cam.fx, m.fy = (float)cam.fy, m.cx = (float)cam.cx, m.cy = (float)cam.cy;
+  m.k1 = (float)cam.d[0], m.k2 = (float)cam.d[1], m.p1 = (float)cam.d[2], m.p2 = (float)cam.d[3], m.k3 = (float)cam.d[4];
+  m.map1 = static_cast<short2*>(c->u_map1.p);
+  m.map2 = static_cast<uint16_t*>(c->u_map2.p);
+  CK(record_event(c->u_map_ev[0], s));
+  CK(undistort_map_launch(m, s));
+  CK(record_event(c->u_map_ev[1], s));
+  c->launches += 1;
+  c->u_cam = cam, c->u_map_pitch = mp, c->u_map_ok = true, c->u_map_built = true;
+  return PLSVO_OK;
+}
+
+// vikit hands the parameters to OpenCV as Mat_<float>: they must stay finite, and fx, fy non-zero, after that rounding
+int check_pinhole_params(plsvo_ctx_impl* c, const plsvo_pinhole_camera& cam, const char* who) {
+  const double par[9] = {cam.fx, cam.fy, cam.cx, cam.cy, cam.d[0], cam.d[1], cam.d[2], cam.d[3], cam.d[4]};
+  for (double p : par)
+    if (!isfinite(p) || !isfinite((float)p)) return fail(c, PLSVO_ERR_INVALID, (std::string(who) + ": a parameter is not finite in float").c_str());
+  if ((float)cam.fx == 0.f || (float)cam.fy == 0.f) return fail(c, PLSVO_ERR_INVALID, (std::string(who) + ": fx and fy must be non-zero").c_str());
+  return PLSVO_OK;
+}
+}  // namespace
+
 // vk::PinholeCamera::undistortImage + createImgPyramid for B frames: raw frames up, map (built once per camera), remap
 // into level 0, pyramid kernel for levels 1.., every level down.
 static int undistort_batch_run_body(plsvo_ctx* ctx, const plsvo_undistort_batch* in, const plsvo_pyramid_result* out) {
@@ -1835,11 +1872,7 @@ static int undistort_batch_run_body(plsvo_ctx* ctx, const plsvo_undistort_batch*
   if (in->n_levels < 1 || in->n_levels > 7) return fail(c, PLSVO_ERR_INVALID, "undistort batch: n_levels must be in [1,7]");
   if (!in->img0) return fail(c, PLSVO_ERR_INVALID, "undistort batch: raw frames missing (img0 is NULL)");
   if (in->pitch0 < (size_t)W) return fail(c, PLSVO_ERR_INVALID, "undistort batch: pitch0 smaller than the image width");
-  // vikit hands the parameters to OpenCV as Mat_<float>: they must stay finite, and fx, fy non-zero, after that rounding
-  const double par[9] = {cam.fx, cam.fy, cam.cx, cam.cy, cam.d[0], cam.d[1], cam.d[2], cam.d[3], cam.d[4]};
-  for (double p : par)
-    if (!isfinite(p) || !isfinite((float)p)) return fail(c, PLSVO_ERR_INVALID, "undistort camera: a parameter is not finite in float");
-  if ((float)cam.fx == 0.f || (float)cam.fy == 0.f) return fail(c, PLSVO_ERR_INVALID, "undistort camera: fx and fy must be non-zero");
+  if (check_pinhole_params(c, cam, "undistort camera") != PLSVO_OK) return PLSVO_ERR_INVALID;
   for (int l = 0; l < in->n_levels; ++l) {
     const int cols = W >> l, rows = H >> l;
     if (cols <= 0 || rows <= 0) return fail(c, PLSVO_ERR_INVALID, "pyramid level smaller than one pixel");
@@ -1877,25 +1910,9 @@ static int undistort_batch_run_body(plsvo_ctx* ctx, const plsvo_undistort_batch*
     for (size_t b = 0; b < B; ++b)
       CK(cudaMemcpy2DAsync(raw + b * a.stride[0], a.pitch[0], in->img0 + b * in->stride0, in->pitch0, W, H, cudaMemcpyHostToDevice, s));
   }
-  if (distortion && (!c->u_map_ok || memcmp(&c->u_cam, &cam, sizeof cam) != 0)) {
-    c->u_map_ok = false;
-    const int mp = (W + kRemapTileW - 1) / kRemapTileW * kRemapTileW;
-    const size_t n = (size_t)H * mp;
-    CK(ensure(c->u_map1, n * sizeof(short2)));
-    CK(ensure(c->u_map2, n * sizeof(uint16_t)));
-    CK(cudaMemsetAsync(c->u_map1.p, 0, n * sizeof(short2), s));  // the row padding: read by whole-tile loads, never used
-    CK(cudaMemsetAsync(c->u_map2.p, 0, n * sizeof(uint16_t), s));
-    UndistortMapArgs m;
-    m.width = W, m.height = H, m.map_pitch = mp;
-    m.fx = (float)cam.fx, m.fy = (float)cam.fy, m.cx = (float)cam.cx, m.cy = (float)cam.cy;
-    m.k1 = (float)cam.d[0], m.k2 = (float)cam.d[1], m.p1 = (float)cam.d[2], m.p2 = (float)cam.d[3], m.k3 = (float)cam.d[4];
-    m.map1 = static_cast<short2*>(c->u_map1.p);
-    m.map2 = static_cast<uint16_t*>(c->u_map2.p);
-    CK(record_event(c->u_map_ev[0], s));
-    CK(undistort_map_launch(m, s));
-    CK(record_event(c->u_map_ev[1], s));
-    c->launches += 1;
-    c->u_cam = cam, c->u_map_pitch = mp, c->u_map_ok = true, c->u_map_built = true;
+  if (distortion) {
+    const int rc = undistort_map_ensure(c, cam, s);
+    if (rc != PLSVO_OK) return rc;
   }
   CK(kernel_timer(c, 0, s));
   if (distortion) {
@@ -1941,6 +1958,152 @@ extern "C" int plsvo_last_map_build_ms(plsvo_ctx* ctx, float* ms) {
   CK(cudaEventSynchronize(c->u_map_ev[1]));
   CK(cudaEventElapsedTime(ms, c->u_map_ev[0], c->u_map_ev[1]));
   return PLSVO_OK;
+}
+
+// plsvo_align_raw_batch_run / plsvo_track_raw_batch_run (pb == NULL: alignment only): raw frames up, the camera's map
+// (cached), one undistort_pyramid_kernel over every frame storing the levels alignment reads and those rect_out asks for,
+// straight into the device layout of the alignment batch, then the alignment (and pose-optimiser) kernels as the plain
+// upload -> launch -> download sequence runs them.  The arrival-gated streamed path is not taken.
+static int raw_run_body(plsvo_ctx* ctx, const plsvo_raw_frames* raw, const plsvo_align_batch* ab, const plsvo_align_params* ap,
+                        const plsvo_poseopt_batch* pb, const plsvo_poseopt_params* pp, const plsvo_align_result* ao,
+                        const plsvo_poseopt_result* po, const plsvo_pyramid_result* rect) {
+  plsvo_ctx_impl* c = CTX(ctx);
+  c->u_map_built = false;
+  const plsvo_pinhole_camera& cam = raw->cam;
+  const int W = cam.width, H = cam.height;
+  if (W <= 0 || H <= 0) return fail(c, PLSVO_ERR_INVALID, "raw frames: width and height must be positive");
+  if (check_pinhole_params(c, cam, "raw-frame camera") != PLSVO_OK) return PLSVO_ERR_INVALID;
+  if (ab->cam.width != W || ab->cam.height != H || ab->cam.fx != cam.fx || ab->cam.fy != cam.fy || ab->cam.cx != cam.cx ||
+      ab->cam.cy != cam.cy)
+    return fail(c, PLSVO_ERR_INVALID, "raw frames: batch->cam and raw->cam differ in width, height, fx, fy, cx or cy");
+  for (int l = 0; l < PLSVO_MAX_LEVELS; ++l)
+    if (ab->ref_img[l] || ab->cur_img[l])
+      return fail(c, PLSVO_ERR_INVALID, "raw frames: image pointers in the alignment batch (the images come from the raw frames only)");
+  const bool chain = (ab->flags & PLSVO_ALIGN_FRAME_CHAIN) != 0;
+  if (!raw->ref_raw || (!chain && !raw->cur_raw)) return fail(c, PLSVO_ERR_INVALID, "raw frames missing (a raw stack is NULL)");
+  if (chain && raw->cur_raw) return fail(c, PLSVO_ERR_INVALID, "raw frames: cur_raw must be NULL with PLSVO_ALIGN_FRAME_CHAIN");
+  if (raw->pitch < (size_t)W) return fail(c, PLSVO_ERR_INVALID, "raw frames: pitch smaller than the image width");
+  if (ap->min_level < 0 || ap->max_level < ap->min_level || ap->n_iter < 1) return fail(c, PLSVO_ERR_INVALID, "level range / n_iter");
+  if (ap->max_level > 6) return fail(c, PLSVO_ERR_INVALID, "raw frames: max_level > 6 (one 64x64 level-0 tile holds levels 0..6)");
+  if (pb && pb->batch != ab->batch) return fail(c, PLSVO_ERR_INVALID, "alignment and pose-optimiser batches differ in size");
+  // the levels the kernel stores: [min_level, max_level] for alignment, and every level rect_out asks for
+  bool want[PLSVO_MAX_LEVELS] = {false};
+  int top = ap->max_level;
+  for (int l = 0; l < PLSVO_MAX_LEVELS; ++l) {
+    const bool out = rect && rect->level[l];
+    want[l] = out || (l >= ap->min_level && l <= ap->max_level);
+    if (!want[l]) continue;
+    if (l > 6) return fail(c, PLSVO_ERR_INVALID, "rect_out: level above 6 (one 64x64 level-0 tile holds levels 0..6)");
+    if ((W >> l) <= 0 || (H >> l) <= 0) return fail(c, PLSVO_ERR_INVALID, "pyramid level smaller than one pixel");
+    if (out && rect->pitch[l] < (size_t)(W >> l)) return fail(c, PLSVO_ERR_INVALID, "rect_out: pitch smaller than the level width");
+    top = std::max(top, l);
+  }
+  // PinholeCamera's distortion_ flag: without it level 0 is the raw frame itself
+  const bool distortion = fabs(cam.d[0]) > 0.0000001;
+  if (!undistort_pyramid_launch || (distortion && !undistort_map_launch))
+    return fail(c, PLSVO_ERR_CUDA, "raw-frame rectification kernels are not linked into this library", cudaErrorNotSupported);
+  // features, poses, outputs and the host-side sizing of the alignment batch (no image is shipped)
+  const size_t B = (size_t)std::max(ab->batch, 0);
+  int rc = align_upload_impl(c, ab, 0, B, c->stream, 1);
+  if (rc != PLSVO_OK) return rc;
+  if (pb) {
+    rc = poseopt_upload_impl(c, pb, pb->T_f_w ? nullptr : c->aa.out_T);
+    if (rc != PLSVO_OK) return rc;
+  }
+  cudaStream_t s = c->stream;
+  AlignArgs& a = c->aa;
+  // every frame in one stack per level: the B+1 frames of a chain, or the B reference frames followed by the B current ones
+  const size_t n_frames = chain ? B + 1 : 2 * B;
+  RawPyramidArgs r;
+  memset(&r, 0, sizeof r);
+  r.B = (int)n_frames, r.width = W, r.height = H, r.n_levels = top + 1;
+  size_t total = 0, off[PLSVO_MAX_LEVELS] = {0};
+  for (int l = 0; l <= top; ++l) {
+    if (!want[l]) continue;
+    r.pitch[l] = (uint32_t)(((W >> l) + 15) / 16 * 16);
+    r.stride[l] = (size_t)(H >> l) * r.pitch[l];
+    total = (total + 255) / 256 * 256;
+    off[l] = total;
+    total += r.stride[l] * n_frames;
+  }
+  CK(ensure(c->d_ref_img, total + 256));
+  for (int l = 0; l <= top; ++l) {
+    if (!want[l]) continue;
+    r.level[l] = static_cast<uint8_t*>(c->d_ref_img.p) + off[l];
+    a.ref_img[l] = r.level[l];
+    a.cur_img[l] = r.level[l] + (chain ? 1 : B) * r.stride[l];
+    a.pitch[l] = r.pitch[l], a.stride[l] = r.stride[l];
+    c->lvl_uploaded[l] = true;  // present: align_derive_levels derives nothing
+  }
+  // raw frames: one linear copy per stack when the host layout is uniform (kept on the device), else frame by frame
+  const bool uniform = raw->stride == (size_t)H * raw->pitch;
+  r.src_pitch = uniform ? raw->pitch : (size_t)W;
+  r.src_stride = uniform ? raw->stride : (size_t)H * W;
+  CK(ensure(c->u_raw, r.src_stride * n_frames));
+  uint8_t* d_raw = static_cast<uint8_t*>(c->u_raw.p);
+  r.src = d_raw;
+  const uint8_t* stacks[2] = {raw->ref_raw, chain ? nullptr : raw->cur_raw};
+  const size_t per_stack = chain ? B + 1 : B;
+  for (int k = 0; k < 2 && stacks[k]; ++k) {
+    uint8_t* dst = d_raw + k * per_stack * r.src_stride;
+    if (uniform) {
+      // the last row of the last frame needs only W of its pitch bytes
+      CK(cudaMemcpyAsync(dst, stacks[k], per_stack * r.src_stride - (raw->pitch - W), cudaMemcpyHostToDevice, s));
+    } else {
+      for (size_t f = 0; f < per_stack; ++f)
+        CK(cudaMemcpy2DAsync(dst + f * r.src_stride, r.src_pitch, stacks[k] + f * raw->stride, raw->pitch, W, H, cudaMemcpyHostToDevice, s));
+    }
+  }
+  if (distortion) {
+    rc = undistort_map_ensure(c, cam, s);
+    if (rc != PLSVO_OK) return rc;
+    r.map_pitch = c->u_map_pitch;
+    r.map1 = static_cast<const short2*>(c->u_map1.p), r.map2 = static_cast<const uint16_t*>(c->u_map2.p);
+  }
+  rc = align_derive_levels(c, ap->min_level, ap->max_level, 0, B, s, false);
+  if (rc != PLSVO_OK) return rc;
+  AlignPlan plan;
+  rc = align_plan(c, ap, (int)B, &plan);
+  if (rc != PLSVO_OK) return rc;
+  CK(kernel_timer(c, 0, s));
+  CK(undistort_pyramid_launch(r, c->num_sms, s));
+  c->launches += 1;
+  rc = align_launch_range(c, plan, 0, B, 0, s);
+  if (rc == PLSVO_OK && pb) rc = plsvo_poseopt_launch(ctx, pp);
+  if (rc != PLSVO_OK) return rc;
+  CK(kernel_timer(c, 1, s));
+  for (int l = 0; l <= top; ++l) {
+    if (!rect || !rect->level[l]) continue;
+    const int cols = W >> l, rows = H >> l;
+    if (rect->stride[l] == (size_t)rows * rect->pitch[l]) {
+      CK(cudaMemcpy2DAsync(rect->level[l], rect->pitch[l], r.level[l], r.pitch[l], cols, (size_t)rows * n_frames, cudaMemcpyDeviceToHost, s));
+    } else {
+      for (size_t f = 0; f < n_frames; ++f)
+        CK(cudaMemcpy2DAsync(rect->level[l] + f * rect->stride[l], rect->pitch[l], r.level[l] + f * r.stride[l], r.pitch[l], cols, rows,
+                             cudaMemcpyDeviceToHost, s));
+    }
+  }
+  if (ao) {
+    rc = plsvo_align_download(ctx, ao);
+    if (rc != PLSVO_OK) return rc;
+  }
+  if (pb) return plsvo_poseopt_download(ctx, po);
+  CK(cudaStreamSynchronize(s));
+  return PLSVO_OK;
+}
+
+extern "C" int plsvo_align_raw_batch_run(plsvo_ctx* ctx, const plsvo_raw_frames* raw, const plsvo_align_batch* b,
+                                         const plsvo_align_params* p, const plsvo_align_result* o, const plsvo_pyramid_result* rect_out) {
+  if (!ctx || !raw || !b || !p || !o) return PLSVO_ERR_INVALID;
+  return settled(CTX(ctx), raw_run_body(ctx, raw, b, p, nullptr, nullptr, o, nullptr, rect_out));
+}
+
+extern "C" int plsvo_track_raw_batch_run(plsvo_ctx* ctx, const plsvo_raw_frames* raw, const plsvo_align_batch* ab,
+                                         const plsvo_align_params* ap, const plsvo_poseopt_batch* pb, const plsvo_poseopt_params* pp,
+                                         const plsvo_align_result* ao, const plsvo_poseopt_result* po,
+                                         const plsvo_pyramid_result* rect_out) {
+  if (!ctx || !raw || !ab || !ap || !pb || !pp || !po) return PLSVO_ERR_INVALID;
+  return settled(CTX(ctx), raw_run_body(ctx, raw, ab, ap, pb, pp, ao, po, rect_out));
 }
 
 extern "C" int plsvo_match_direct_batch_run(plsvo_ctx* ctx, const plsvo_match_batch* in, const plsvo_match_result* out) {

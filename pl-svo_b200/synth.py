@@ -554,6 +554,59 @@ def make_chain_batch(cam: Camera = VGA, batch: int = 8, n_pts: int = 300, n_segs
                             T_ref_w_gt=poses[:-1], T_cur_w_gt=poses[1:], chain=True, **kw)
 
 
+# EuRoC's cam0 as config/dataset_params.yaml gives it: the undistorted pinhole camera and its Brown-Conrady coefficients
+# (k1, k2, p1, p2, k3) = vk::PinholeCamera's d0..d4
+EUROC = Camera(752, 480, 416.401549, 416.375319, 385.554786, 237.640332)
+EUROC_DIST = (-0.27797, 0.060647, -0.002097, 0.000373, 0.0)
+
+
+def undistort_points(cam: Camera, dist, u: torch.Tensor, v: torch.Tensor, iters: int = 20):
+    """cv::undistortPoints for raw pixels (u, v) of the distorted pinhole camera `cam` with (k1, k2, p1, p2, k3) = dist:
+    OpenCV's fixed-point iteration x = (x0 - delta(x)) / radial(x), in float64 -> normalised undistorted (x, y)."""
+    k1, k2, p1, p2, k3 = (float(d) for d in dist)
+    x0, y0 = (u - cam.cx) / cam.fx, (v - cam.cy) / cam.fy
+    x, y = x0.clone(), y0.clone()
+    for _ in range(iters):
+        r2 = x * x + y * y
+        icdist = 1.0 / (1.0 + ((k3 * r2 + k2) * r2 + k1) * r2)
+        dx = 2.0 * p1 * x * y + p2 * (r2 + 2.0 * x * x)
+        dy = p1 * (r2 + 2.0 * y * y) + 2.0 * p2 * x * y
+        x, y = (x0 - dx) * icdist, (y0 - dy) * icdist
+    return x, y
+
+
+def render_distorted(scene: Scene, cam: Camera, dist, pose7: torch.Tensor, chunk: int = 64) -> torch.Tensor:
+    """Raw frames of the analytic scene as a lens with Brown-Conrady distortion `dist` sees it: pose7 [B,7] (T_f_w) ->
+    u8 [B,H,W].  Each raw pixel's ray is its undistorted normalised coordinate (undistort_points), so rectifying these
+    frames with PinholeCamera(cam, *dist).undistortImage approximates Scene.render(cam, pose7) away from the border."""
+    dev = pose7.device
+    B = pose7.shape[0]
+    u = torch.arange(cam.width, dtype=torch.float64, device=dev)
+    v = torch.arange(cam.height, dtype=torch.float64, device=dev)
+    vv, uu = torch.meshgrid(v, u, indexing="ij")
+    x, y = undistort_points(cam, dist, uu, vv)
+    dirs = torch.stack([x, y, torch.ones_like(x)], -1).reshape(1, -1, 3)
+    out = torch.empty(B, cam.height, cam.width, dtype=torch.uint8, device=dev)
+    for s in range(0, B, chunk):
+        R, t = pose7_to_Rt(pose7[s : s + chunk])
+        P = scene.intersect(R, t, dirs.expand(R.shape[0], -1, -1))
+        I = scene.texture(P[..., 0], P[..., 1])
+        out[s : s + chunk] = I.round().clamp(0, 255).to(torch.uint8).reshape(-1, cam.height, cam.width)
+    return out
+
+
+def make_raw_chain_batch(cam: Camera = EUROC, dist=EUROC_DIST, batch: int = 8, n_pts: int = 300, n_segs: int = 80,
+                         seed: int = 3000, device: str | torch.device = "cpu", scene: Scene | None = None, **kw):
+    """make_chain_batch whose frames are also rendered raw through a distorting lens: returns (AlignData, raw u8
+    [B+1,H,W]).  Features, poses and ground truth are those of the undistorted camera `cam` (what the pipeline's
+    handler sees after rectification); the AlignData's own pyramids are Scene.render's undistorted frames."""
+    scene = scene or Scene()
+    data = make_chain_batch(cam=cam, batch=batch, n_pts=n_pts, n_segs=n_segs, seed=seed, device=device, scene=scene, **kw)
+    poses = torch.tensor(np.concatenate([data.T_ref_w, data.T_cur_w_gt[-1:]], 0), dtype=torch.float64, device=torch.device(device))
+    raw = render_distorted(scene, cam, dist, poses)
+    return data, np.ascontiguousarray(raw.cpu().numpy())
+
+
 def run_sequence(poses, steps, track_fn):
     """The frame-to-frame chain of FrameHandlerMono::processFrame (src/frame_handler_mono.cpp:263-340) over a sequence:
     new_frame.T_f_w = last_frame.T_f_w (:266), sparse image alignment, pose optimisation, and the result becomes the
