@@ -184,18 +184,23 @@ def check(out, data_as_kernel_sees_it, what=""):
     assert np.array_equal(out.patch_iters, np.broadcast_to(npt, out.patch_iters.shape)), what
 
 
-def run(data, ctx=None, **envs):
+def run(data, ctx=None, three_leg=False, **envs):
+    """One plsvo_align_batch_run call, or (three_leg) the plsvo_align_upload / _launch / _download sequence."""
     with env(**envs):
         al = pkg.SparseImgAlign(data.max_level, data.min_level, 30, ctx=ctx or pkg.api.Context(0))
-        return al.run(data)
+        if not three_leg:
+            return al.run(data)
+        al.upload(data)
+        al.launch()
+        return al.download()
 
 
 # ---- scenarios ----
 def s_plain_upload_launch_download():
     d = make_batch(5, 40, 9, 1)
-    check(run(d, PLSVO_E2E_CHUNKS=1, PLSVO_NO_SMALL_UPLOAD=1), d, "plain")
+    check(run(d, PLSVO_NO_SMALL_UPLOAD=1), d, "plain")
     d = make_batch(6, 33, 0, 2)  # no segments at all
-    check(run(d, PLSVO_E2E_CHUNKS=1, PLSVO_NO_SMALL_UPLOAD=1), d, "points only")
+    check(run(d, PLSVO_NO_SMALL_UPLOAD=1), d, "points only")
 
 
 def s_small_batch_staging_block():
@@ -242,18 +247,10 @@ def s_three_leg_api_and_relaunch():
     check(al.download(), d, "relaunch, derived levels")
 
 
-def s_k_kernel_pipeline():
-    d = make_batch(26, 30, 8, 40, ragged=True)
-    for k in (2, 3, 8):
-        check(run(d, PLSVO_E2E_CHUNKS=k, PLSVO_NO_SMALL_UPLOAD=1), d, f"chunks={k}")
-        check(run(shipped(d, [2]), PLSVO_E2E_CHUNKS=k, PLSVO_NO_SMALL_UPLOAD=1), d, f"chunks={k}, derived levels")
-
-
 def s_arrival_gated_stream():
     d = make_batch(300, 24, 6, 50, ragged=True)
     full_bytes = None
-    for envs in ({}, {"PLSVO_GATE_CHUNK": 128}, {"PLSVO_GATE_CHUNK": 128, "PLSVO_COPY_STREAMS": 2}, {"PLSVO_GATE_INTERLEAVED": 1},
-                 {"PLSVO_GATE_CHUNK": 128, "PLSVO_GATE_INTERLEAVED": 1, "PLSVO_COPY_STREAMS": 3}):
+    for envs in ({}, {"PLSVO_GATE_CHUNK": 128}):
         h0 = lib.fake_cuda_h2d_bytes()
         check(run(d, **envs), d, f"gated {envs}")
         n_chunks = -(-d.batch // int(envs.get("PLSVO_GATE_CHUNK", 256)))
@@ -279,9 +276,8 @@ def s_padded_host_layouts():
                 big = np.full((n, h + (layout != "row_padded"), w + 3 * (layout != "frame_padded")), 255, np.uint8)
                 big[:, :h, :w] = src[l]
                 dst[l] = big[:, :h, :w]
-        for k in (1, 2):
-            check(run(p, PLSVO_E2E_CHUNKS=k), d, f"{layout}, chunks={k}")
-            check(run(p, PLSVO_E2E_CHUNKS=k, PLSVO_NO_SMALL_UPLOAD=1), d, f"{layout}, chunks={k}, plain copies")
+        check(run(p), d, layout)
+        check(run(p, PLSVO_NO_SMALL_UPLOAD=1), d, f"{layout}, plain copies")
 
 
 def s_lean_features():
@@ -293,10 +289,9 @@ def s_lean_features():
 
 
 def s_chain_every_host_path():
-    # small block / plain copies / k-kernel pipeline, all levels shipped or derived
+    # small block / plain copies, all levels shipped or derived (the arrival-gated stream: s_chain_arrival_gated_stream)
     d = make_batch(26, 30, 8, 80, chain=True, ragged=True)
-    for envs in ({}, {"PLSVO_NO_SMALL_UPLOAD": 1}, {"PLSVO_NO_SMALL_UPLOAD": 1, "PLSVO_E2E_CHUNKS": 1}, {"PLSVO_E2E_CHUNKS": 3},
-                 {"PLSVO_E2E_CHUNKS": 3, "PLSVO_NO_SMALL_UPLOAD": 1}, {"PLSVO_E2E_CHUNKS": 8, "PLSVO_NO_SMALL_UPLOAD": 1}):
+    for envs in ({}, {"PLSVO_NO_SMALL_UPLOAD": 1}):
         check(run(one_stack(d), **envs), d, f"chain {envs}")
         check(run(one_stack(d, [2]), **envs), d, f"chain, derived levels {envs}")
     d = make_batch(3, 30, 8, 81, chain=True)
@@ -315,7 +310,7 @@ def s_chain_every_host_path():
 def s_chain_arrival_gated_stream():
     d = make_batch(300, 24, 6, 90, chain=True)
     two_stack_bytes = None
-    for envs in ({}, {"PLSVO_GATE_CHUNK": 128}, {"PLSVO_GATE_CHUNK": 128, "PLSVO_COPY_STREAMS": 2}, {"PLSVO_GATE_INTERLEAVED": 1}):
+    for envs in ({}, {"PLSVO_GATE_CHUNK": 128}):
         for levels in (LEVELS, (2,)):
             h0 = lib.fake_cuda_h2d_bytes()
             check(run(shipped(d, levels), **envs), d, f"two stacks {envs} {levels}")
@@ -344,8 +339,7 @@ def s_chain_padded_host_layouts():
             big = np.full((n, h + (layout == "frame_padded"), w + 3 * (layout == "row_padded")), 255, np.uint8)
             big[:, :h, :w] = f
             o.frame_pyr[l] = big[:, :h, :w]
-        for k in (1, 2, 3):
-            check(run(o, PLSVO_E2E_CHUNKS=k), d, f"chain {layout} chunks={k}")
+        check(run(o), d, f"chain {layout}")
     # a chain whose frames are not 128-byte multiples must leave the gated path (QVGA level 4: 20 x 15 bytes)
     q = make_batch(260, 12, 3, 101, cam=synth.QVGA, chain=True)
     check(run(one_stack(q)), q, "chain with unaligned frames")
@@ -480,7 +474,7 @@ def padded_view(stack, layout, rng):
 def s_randomised_configurations():
     """Differential test over random corners of the configuration space: camera size, level range, which levels are shipped,
     batch size on either side of the streaming threshold, feature counts down to none, ragged counts, masks, lean features,
-    frame chains, padded host layouts, and the environment switches that select the host path."""
+    frame chains, padded host layouts, the one-call and three-leg forms, and the environment switches of the host path."""
     rng = np.random.default_rng(int(os.environ.get("PLSVO_FUZZ_SEED", 2024)))  # PLSVO_FUZZ_SEED / _ITERS: longer hunts by hand
     cams = [synth.Camera(w, h, 0.7 * w, 0.7 * w, w / 2 - 0.5, h / 2 - 0.5) for w, h in ((128, 96), (256, 192), (384, 128), (640, 480))]
     ctx = pkg.api.Context(0)  # one context for everything: every call inherits the buffers of a differently shaped one
@@ -511,13 +505,13 @@ def s_randomised_configurations():
                 seed_pad = int(rng.integers(0, 1 << 30))
                 call.ref_pyr = {l: padded_view(f, layout, np.random.default_rng(seed_pad + l)) for l, f in call.ref_pyr.items()}
                 call.cur_pyr = {l: padded_view(f, layout, np.random.default_rng(seed_pad + l)) for l, f in call.cur_pyr.items()}
-        envs = [{}, {}, {"PLSVO_NO_SMALL_UPLOAD": 1}, {"PLSVO_E2E_CHUNKS": int(rng.integers(1, 6))},
-                {"PLSVO_E2E_CHUNKS": int(rng.integers(2, 9)), "PLSVO_NO_SMALL_UPLOAD": 1}, {"PLSVO_GATE_CHUNK": 128},
-                {"PLSVO_GATE_CHUNK": 128, "PLSVO_COPY_STREAMS": int(rng.integers(2, 5))}, {"PLSVO_GATE_INTERLEAVED": 1}][int(rng.integers(0, 8))]
+        pick = int(rng.integers(0, 8))  # one call or three legs, with and without the small block, gate chunk 256 or 128
+        three_leg = bool(pick & 1)
+        envs = {**({"PLSVO_NO_SMALL_UPLOAD": 1} if pick & 2 else {}), **({"PLSVO_GATE_CHUNK": 128} if pick & 4 else {})}
         what = (f"#{it}: {cam.width}x{cam.height} levels {min_level}..{max_level} shipped {levels} B={B} pts={n_pts} segs={n_segs} chain={chain} "
-                f"layout={layout} lean={seen is not d or hasattr(d, 'pt_depth') and d.pt_depth is not None} env={envs}")
+                f"layout={layout} lean={seen is not d or hasattr(d, 'pt_depth') and d.pt_depth is not None} three_leg={three_leg} env={envs}")
         try:
-            out = run(call, ctx=ctx, **envs)
+            out = run(call, ctx=ctx, three_leg=three_leg, **envs)
         except pkg.api.PlsvoError as ex:
             raise AssertionError(f"{what}: {ex}") from None
         check(out, seen, what)

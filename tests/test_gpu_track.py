@@ -120,13 +120,13 @@ def test_feature_counts_out_of_range_are_rejected(pkg, synth, gen_device):
 
 
 def test_gate_with_several_chunks_and_copy_streams(pkg, synth, gen_device, monkeypatch):
-    """The arrival gate with more than one chunk and round-robin copy streams (PLSVO_GATE_CHUNK=128, 3 chunks)."""
+    """The arrival gate with more than one chunk on the copy stream (PLSVO_GATE_CHUNK=128, 3 chunks)."""
     data = synth.make_align_batch(batch=300, n_pts=64, n_segs=12, device=gen_device, seed=6600)
-    monkeypatch.setenv("PLSVO_E2E_CHUNKS", "1")
-    plain = pkg.SparseImgAlign(4, 2, 30).run(data)
-    monkeypatch.delenv("PLSVO_E2E_CHUNKS")
+    al = pkg.SparseImgAlign(4, 2, 30)
+    al.upload(data)  # the plain upload -> launch -> download sequence
+    al.launch()
+    plain = al.download()
     monkeypatch.setenv("PLSVO_GATE_CHUNK", "128")
-    monkeypatch.setenv("PLSVO_COPY_STREAMS", "2")
     monkeypatch.setenv("PLSVO_VARIANT", "128,4")  # the CTA shape of the single-shot call: bitwise comparison of the gate alone
     for _ in range(2):
         gated = pkg.SparseImgAlign(4, 2, 30).run(data)

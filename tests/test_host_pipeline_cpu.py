@@ -1,7 +1,7 @@
 """The host side of the C ABI, exercised without a GPU.
 
 `pl-svo_b200/csrc/plsvo_abi.cu` is pure host code (buffer sizing, upload planning, the small-batch staging block, the
-k-kernel pipeline, the arrival-gated stream, device-side pyramid derivation, the frame-chain layout, error exits).  On a
+arrival-gated stream, device-side pyramid derivation, the frame-chain layout, error exits).  On a
 GPU box it is covered by the `-m gpu` parity tests; here it is compiled UNCHANGED as C++ and linked against a
 single-threaded model of the CUDA runtime (tests/hostmodel/fake_cudart.cpp: FIFO streams that run as lazily — or, in a
 second pass, as eagerly — as events and the arrival gate allow, poisoned and bounds-checked "device" memory) and against
@@ -11,8 +11,9 @@ the same digests computed in NumPy from the caller's arrays: whichever host path
 exactly the caller's bytes, every buffer must be large enough, every dependency must be expressed, and no copy from the
 caller's arrays may be pending when a call returns.
 
-The second half seeds faults into a copy of plsvo_abi.cu (a dropped event wait, an undersized frame stack, a frame that is
-never shipped, an arrival flag raised too early, a missing drain on an error exit) and requires the model to notice each of them.
+The second half seeds faults into a copy of plsvo_abi.cu (a dropped wait for the arrival of the copies, an undersized frame
+stack, a frame that is never shipped, an arrival flag raised too early, a missing drain on an error exit) and requires the
+model to notice each of them.
 
 Nothing here is a parity statement about the CUDA kernels — that is what the `-m gpu` tests are for."""
 import importlib.util
@@ -28,7 +29,6 @@ HM = os.path.join(HERE, "hostmodel")
 ABI_SOURCE = os.path.join(os.path.dirname(HERE), "pl-svo_b200", "csrc", "plsvo_abi.cu")
 
 SCENARIOS = ["plain_upload_launch_download", "small_batch_staging_block", "staging_block_grows_while_a_copy_is_queued", "three_leg_api_and_relaunch",
-             "k_kernel_pipeline",
              "arrival_gated_stream", "padded_host_layouts", "lean_features", "chain_every_host_path", "chain_arrival_gated_stream",
              "chain_padded_host_layouts", "rejected_inputs_leave_nothing_in_flight", "forced_variant_is_the_only_one_tried",
              "pose_optimiser_host_paths", "pyramid_call",
@@ -109,10 +109,10 @@ def test_fast_gpu_tier_files_against_the_host_model_with_oracle_backed_kernels(h
 
 # ---- the model must notice seeded faults -------------------------------------------------------------------------------
 FAULTS = {
-    # the k-kernel pipeline forgets to make the kernel of a chunk wait for that chunk's copies
+    # the streamed kernel is launched without its arrival gate: it does not wait for the copies of a chunk to land
     "dropped_event_wait": (
-        "    CK(cudaStreamWaitEvent(c->stream, c->chunk_ev[k], 0));\n", "",
-        "lazy", ["k_kernel_pipeline"]),
+        "  rc = align_launch_kernel(c, plan, c->stream, chunk);  // gated on arrivals\n", "  rc = align_launch_kernel(c, plan, c->stream, 0);\n",
+        "lazy", ["arrival_gated_stream"]),
     # a frame chain sized like a two-stack batch: B frames instead of B + 1
     "undersized_frame_stack": (
         "    const size_t n_frames = B + (c->chain ? 1 : 0);\n", "    const size_t n_frames = B;\n",
@@ -123,9 +123,9 @@ FAULTS = {
         "lazy", ["chain_arrival_gated_stream"]),
     # the arrival flag of a chunk is raised before the chunk's images have been queued
     "arrival_flag_too_early": (
-        "    for (int k = 0; k < n_chunks; ++k) {\n      c->rr_n = n_rr > 1 ? n_rr : 0, c->rr_i = 0;\n",
-        "    for (int k = 0; k < n_chunks; ++k) {\n      c->rr_n = n_rr > 1 ? n_rr : 0, c->rr_i = 0;\n"
-        "      CK(cudaMemcpyAsync(d_arrived, &c->h_flags[k], sizeof(unsigned int), cudaMemcpyHostToDevice, c->copy_stream));\n",
+        "  for (int k = 0; k < n_chunks; ++k) {\n    const size_t b0 = (size_t)k * chunk, b1 = std::min<size_t>(b0 + chunk, B);\n",
+        "  for (int k = 0; k < n_chunks; ++k) {\n    const size_t b0 = (size_t)k * chunk, b1 = std::min<size_t>(b0 + chunk, B);\n"
+        "    CK(cudaMemcpyAsync(d_arrived, &c->h_flags[k], sizeof(unsigned int), cudaMemcpyHostToDevice, c->copy_stream));\n",
         "lazy", ["arrival_gated_stream"]),
     # error exits return while copies from the caller's arrays are still queued
     "error_exit_without_drain": (

@@ -89,14 +89,14 @@ def with_levels(data, rect, lo, hi, chain):
     return d
 
 
-def host_path_align(pkg, monkeypatch, cam, raw, data, hi, lo, ctx):
-    """plsvo_undistort_batch_run, then plsvo_align_batch_run's plain host-buffer path on the rectified levels."""
+def host_path_align(pkg, cam, raw, data, hi, lo, ctx):
+    """plsvo_undistort_batch_run, then the plain upload -> launch -> download sequence on the rectified levels."""
     frames = raw if not isinstance(raw, tuple) else np.concatenate(raw, 0)
     rect = cam.undistortImage(frames, hi + 1, ctx)
-    monkeypatch.setenv("PLSVO_E2E_CHUNKS", "1")
-    out = pkg.SparseImgAlign(hi, lo, 30, ctx=ctx).run(with_levels(data, rect, lo, hi, not isinstance(raw, tuple)))
-    monkeypatch.delenv("PLSVO_E2E_CHUNKS")
-    return out, rect
+    al = pkg.SparseImgAlign(hi, lo, 30, ctx=ctx)
+    al.upload(with_levels(data, rect, lo, hi, not isinstance(raw, tuple)))
+    al.launch()
+    return al.download(), rect
 
 
 def assert_same(a, b, fields):
@@ -195,13 +195,13 @@ CASES = [  # camera, B, chain, (max_level, min_level)
 
 @pytest.mark.gpu
 @pytest.mark.parametrize("name,B,chain,lv", CASES)
-def test_gpu_align_raw_is_undistort_then_align(pkg, synth, monkeypatch, name, B, chain, lv):
+def test_gpu_align_raw_is_undistort_then_align(pkg, synth, name, B, chain, lv):
     hi, lo = lv
     ctx = pkg.api.Context(0)
     data = features(synth, name, B, seed=B + hi, max_level=hi, min_level=lo)
     raw = raw_frames(name, B + 1, seed=B) if chain else (raw_frames(name, B, seed=B), raw_frames(name, B, seed=B + 1))
     cam = camera(pkg, name)
-    want, _ = host_path_align(pkg, monkeypatch, cam, raw, data, hi, lo, ctx)
+    want, _ = host_path_align(pkg, cam, raw, data, hi, lo, ctx)
     got = pkg.SparseImgAlign(hi, lo, 30, ctx=ctx).run_raw(cam, raw, data)
     assert_same(got, want, ALIGN_FIELDS)
     assert ctx.last_kernel_ms() >= 0
@@ -210,7 +210,7 @@ def test_gpu_align_raw_is_undistort_then_align(pkg, synth, monkeypatch, name, B,
 
 @pytest.mark.gpu
 @pytest.mark.parametrize("chain", [True, False])
-def test_gpu_padded_and_strided_raw_rows(pkg, synth, monkeypatch, chain):
+def test_gpu_padded_and_strided_raw_rows(pkg, synth, chain):
     B, W, H = 5, *params(EUROC)[:2]
     ctx = pkg.api.Context(0)
     data = features(synth, EUROC, B, seed=71)
@@ -220,7 +220,7 @@ def test_gpu_padded_and_strided_raw_rows(pkg, synth, monkeypatch, chain):
     for ref, cur in ((big[: B + 1], big[B + 1 : 2 * B + 1]), (big[::2][: B + 1], big[1::2][:B])):
         raw = ref if chain else (ref[:B], cur)
         assert ref.strides[1] != W
-        want, _ = host_path_align(pkg, monkeypatch, cam, raw, data, 4, 2, ctx)
+        want, _ = host_path_align(pkg, cam, raw, data, 4, 2, ctx)
         got = pkg.SparseImgAlign(4, 2, 30, ctx=ctx).run_raw(cam, raw, data)
         assert_same(got, want, ALIGN_FIELDS)
     ctx.close()
@@ -229,7 +229,7 @@ def test_gpu_padded_and_strided_raw_rows(pkg, synth, monkeypatch, chain):
 @pytest.mark.gpu
 @pytest.mark.parametrize("n_iter_ref", [None, 3])
 @pytest.mark.parametrize("name,B,chain", [(EUROC, 3, True), (ODD, 3, False), (COPY, 2, True), (EUROC, 256, True)])
-def test_gpu_track_raw_is_undistort_then_track(pkg, synth, monkeypatch, name, B, chain, n_iter_ref):
+def test_gpu_track_raw_is_undistort_then_track(pkg, synth, name, B, chain, n_iter_ref):
     ctx = pkg.api.Context(0)
     data = features(synth, name, B, seed=90 + B)
     W, H, fx, fy, cx, cy = params(name)[:6]
@@ -238,7 +238,6 @@ def test_gpu_track_raw_is_undistort_then_track(pkg, synth, monkeypatch, name, B,
     cam = camera(pkg, name)
     frames = raw if chain else np.concatenate(raw, 0)
     rect = cam.undistortImage(frames, 5, ctx)
-    monkeypatch.setenv("PLSVO_E2E_CHUNKS", "1")
     want_a, want_p = pkg.api.track(with_levels(data, rect, 2, 4, chain), po, po_n_iter_ref=n_iter_ref, ctx=ctx)
     got_a, got_p = pkg.track_raw(cam, raw, data, po, po_n_iter_ref=n_iter_ref, ctx=ctx)
     assert_same(got_a, want_a, ALIGN_FIELDS)
@@ -292,7 +291,7 @@ def test_gpu_raw_path_against_the_oracle_end_to_end(pkg, abi, synth, oracle, gen
 
 
 @pytest.mark.gpu
-def test_gpu_context_reuse_cameras_and_sizes(pkg, synth, monkeypatch):
+def test_gpu_context_reuse_cameras_and_sizes(pkg, synth):
     """raw -> plain -> raw on one context, two cameras alternating, an image-size change; the map-build time is reported
     exactly when a call built a map."""
     ctx = pkg.api.Context(0)
@@ -304,7 +303,7 @@ def test_gpu_context_reuse_cameras_and_sizes(pkg, synth, monkeypatch):
         cam = camera(pkg, name)
         got = pkg.SparseImgAlign(4, 2, 30, ctx=ctx).run_raw(cam, raw, data)
         built.append(ctx.last_map_build_ms() is not None)
-        want, _ = host_path_align(pkg, monkeypatch, cam, raw, data, 4, 2, ctx)  # a plain call between raw calls
+        want, _ = host_path_align(pkg, cam, raw, data, 4, 2, ctx)  # a plain call between raw calls
         assert_same(got, want, ALIGN_FIELDS)
     assert built == [True, False, True, True, True, False, True]
     ctx.close()

@@ -2,7 +2,7 @@
 (frame b, frame b+1), as FrameHandlerMono aligns them (src/frame_handler_mono.cpp:176,272) — ships ONE stack of B+1 frames
 instead of a reference stack and a current stack.  The kernel is the same; only the upload differs, so every output must be
 bit-identical to the two-stack form of the same batch on every host path (small-batch block, plain copies, repack of padded
-layouts, chunked pipeline, arrival-gated stream, levels derived on the device), and parity with the oracle follows.
+layouts, arrival-gated stream, levels derived on the device), and parity with the oracle follows.
 """
 import copy
 
@@ -53,13 +53,12 @@ def test_frame_chain_three_leg_api(pkg, synth, gen_device):
     _same(two, al.download())
 
 
-@pytest.mark.parametrize("chunks", ["1", "3"])
-def test_frame_chain_plain_and_chunked_copies(pkg, synth, gen_device, monkeypatch, chunks):
-    """Plain per-array copies (the small-batch staging block disabled) and the k-kernel pipeline: chunk k ships frames
-    (b0, b1] and its kernel reads frames [b0, b1]."""
+@pytest.mark.parametrize("no_small_upload", [None, "1"])
+def test_frame_chain_small_block_and_plain_copies(pkg, synth, gen_device, monkeypatch, no_small_upload):
+    """The small-batch staging block, and plain per-array copies with the block disabled."""
     data = synth.make_chain_batch(batch=26, n_pts=120, n_segs=24, device=gen_device, seed=5220)
-    monkeypatch.setenv("PLSVO_NO_SMALL_UPLOAD", "1")
-    monkeypatch.setenv("PLSVO_E2E_CHUNKS", chunks)
+    if no_small_upload:
+        monkeypatch.setenv("PLSVO_NO_SMALL_UPLOAD", no_small_upload)
     al = pkg.SparseImgAlign(4, 2, 30)
     _same(al.run(data), al.run(_chain(synth, data)))
 
@@ -67,13 +66,10 @@ def test_frame_chain_plain_and_chunked_copies(pkg, synth, gen_device, monkeypatc
 def test_frame_chain_levels_derived_on_the_device(pkg, synth, gen_device, monkeypatch):
     """Only the finest level is shipped; levels 3 and 4 of the B+1 frames come from the pyramid kernel."""
     data = synth.make_chain_batch(batch=20, n_pts=120, n_segs=24, device=gen_device, seed=5230)
-    monkeypatch.setenv("PLSVO_E2E_CHUNKS", "1")
     al = pkg.SparseImgAlign(4, 2, 30)
     full = al.run(data)
     _same(full, al.run(_chain(synth, data, levels=[2])))
     monkeypatch.setenv("PLSVO_NO_SMALL_UPLOAD", "1")
-    _same(full, al.run(_chain(synth, data, levels=[2])))
-    monkeypatch.setenv("PLSVO_E2E_CHUNKS", "4")
     _same(full, al.run(_chain(synth, data, levels=[2])))
 
 
@@ -95,9 +91,6 @@ def test_frame_chain_padded_host_layouts(pkg, synth, gen_device, monkeypatch, la
             big[:, :h, :] = f
             one.frame_pyr[l] = big[:, :h, :]
         assert not one.frame_pyr[l].flags["C_CONTIGUOUS"]
-    monkeypatch.setenv("PLSVO_E2E_CHUNKS", "1")
-    _same(two, pkg.SparseImgAlign(4, 2, 30).run(one))
-    monkeypatch.setenv("PLSVO_E2E_CHUNKS", "2")
     _same(two, pkg.SparseImgAlign(4, 2, 30).run(one))
 
 
@@ -107,9 +100,10 @@ def test_frame_chain_arrival_gated_stream(pkg, synth, gen_device, monkeypatch, g
     takes a pair once frame b+1 has landed and halfSamples both of its frames; the neighbour pair forms the same bytes."""
     data = synth.make_chain_batch(batch=300, n_pts=64, n_segs=12, device=gen_device, seed=5250)
     monkeypatch.setenv("PLSVO_VARIANT", "128,4")  # same CTA shape on every path: bitwise comparison
-    monkeypatch.setenv("PLSVO_E2E_CHUNKS", "1")
-    plain = pkg.SparseImgAlign(4, 2, 30).run(data)
-    monkeypatch.delenv("PLSVO_E2E_CHUNKS")
+    al = pkg.SparseImgAlign(4, 2, 30)
+    al.upload(data)  # the plain upload -> launch -> download sequence
+    al.launch()
+    plain = al.download()
     if gate_chunk:
         monkeypatch.setenv("PLSVO_GATE_CHUNK", gate_chunk)
     al = pkg.SparseImgAlign(4, 2, 30)

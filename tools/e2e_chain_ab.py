@@ -55,7 +55,6 @@ for label, env in (("variant_128_4", {"PLSVO_VARIANT": "128,4"}), ("variant_160_
         os.environ.pop(k)
     res["one_stack_knobs"][label] = {"ms_p50": round(float(np.median(t)), 3), "ms_min": round(float(min(t)), 3)}
 # the plain sequence of the one-stack call: upload, kernel, download, each synchronised
-os.environ["PLSVO_E2E_CHUNKS"] = "1"
 for name, d in (("two_stacks", two), ("one_stack", one)):
     for _ in range(2):
         t0 = time.perf_counter(); al.upload(d); ctx.sync(); t1 = time.perf_counter(); al.launch(); ctx.sync(); t2 = time.perf_counter(); al.download(); t3 = time.perf_counter()

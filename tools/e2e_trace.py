@@ -27,7 +27,6 @@ for gate in os.environ.get("TRACE_GATES", "256").split(","):
     for _ in range(10): al.run(data)
     dt10 = (time.perf_counter() - t0) / 10
     print(json.dumps({"gate": gate, "ms_traced": round(dt * 1e3, 3), "ms": round(dt10 * 1e3, 3), "pairs_per_s": round(B / dt10), "bytes": nbytes}), flush=True)
-os.environ["PLSVO_E2E_CHUNKS"] = "1"
 for _ in range(2):
     t0 = time.perf_counter(); al.upload(data); ctx.sync(); t1 = time.perf_counter(); al.launch(); ctx.sync(); t2 = time.perf_counter(); al.download(); t3 = time.perf_counter()
 print(json.dumps({"single_shot": {"upload_ms": round((t1-t0)*1e3,3), "h2d_gbs": round(nbytes/(t1-t0)/1e9, 1), "kernel_ms": round((t2-t1)*1e3,3), "download_ms": round((t3-t2)*1e3,3)}}))

@@ -1,4 +1,4 @@
-"""e2e (host buffers -> C ABI -> host results) timing vs number of pipeline chunks."""
+"""e2e (host buffers -> C ABI -> host results) timing vs the arrival gate's chunk size (PLSVO_GATE_CHUNK)."""
 import json, os, sys, time
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path[:0] = [ROOT]
@@ -22,19 +22,14 @@ if os.environ.get("TUNE_LEAN", "1") == "1":  # what bench.py's e2e leg ships: fi
     print(json.dumps({"lean_bytes_per_step": nbytes}))
 ctx = plsvo_b200.Context(0)
 al = plsvo_b200.SparseImgAlign(4, 2, 30, ctx=ctx)
-for chunks, gate, rr in ((0, 512, 1), (0, 512, 2), (0, 512, 3), (0, 512, 4), (0, 256, 1), (0, 256, 2), (0, 256, 3), (0, 256, 4),
-                         (0, 128, 4), (0, 384, 3), (1, 0, 1)):
+for gate in (128, 256, 384, 512):
     os.environ['PLSVO_GATE_CHUNK'] = str(gate)
-    os.environ['PLSVO_COPY_STREAMS'] = str(rr)
-    os.environ["PLSVO_E2E_CHUNKS"] = str(chunks) if chunks else ""
-    if not chunks: os.environ.pop("PLSVO_E2E_CHUNKS")
     for _ in range(3): al.run(data)
     t0 = time.perf_counter()
     n = 10
     for _ in range(n): al.run(data)
     dt = (time.perf_counter() - t0) / n
-    print(json.dumps({"chunks": chunks, "gate": gate, "copy_streams": rr, "ms": round(dt * 1e3, 3), "pairs_per_s": round(B / dt)}), flush=True)
-# breakdown of the single-shot path
-os.environ["PLSVO_E2E_CHUNKS"] = "1"
+    print(json.dumps({"gate": gate, "ms": round(dt * 1e3, 3), "pairs_per_s": round(B / dt)}), flush=True)
+# breakdown of the plain upload -> launch -> download sequence
 t0 = time.perf_counter(); al.upload(data); ctx.sync(); t1 = time.perf_counter(); al.launch(); ctx.sync(); t2 = time.perf_counter(); al.download(); t3 = time.perf_counter()
 print(json.dumps({"upload_ms": round((t1-t0)*1e3,3), "launch_ms": round((t2-t1)*1e3,3), "download_ms": round((t3-t2)*1e3,3)}))
