@@ -43,16 +43,26 @@ namespace {
 #ifdef PLSVO_PHASE_CLOCKS
 // Opt-in cycle attribution (build_variant("phase", ["PLSVO_PHASE_CLOCKS"]), never the product build): lane 0 of every
 // warp adds the clock64() cycles since its previous mark to the phase the mark closes; the sums over the grid are read
-// with plsvo_phase_clocks() (tools/phase_clocks.py).  Every mark sits where its warp is converged.
-enum { kPhSetup, kPhPtEval, kPhPtChi2, kPhSeg, kPhReduce, kPhSerial, kPhPair, kNumPhases };
+// with plsvo_phase_clocks() (tools/phase_clocks.py).  Every mark sits where its warp is converged.  The serial section
+// of a pass is split by what its warps do: the cross-warp sum of the partials and the solve (warp 0), the chi2 walk
+// (walker warp), the segment-chi2 sum (segment warp), the wait at the named barrier that joins them, the decision
+// (thread 0) and the block barrier that ends the pass (every warp; the only serial phase of the other warps).
+enum {
+  kPhSetup, kPhPtEval, kPhPtChi2, kPhSeg, kPhReduce,
+  kPhSerRed, kPhSerSolve, kPhSerWalk, kPhSerSegSum, kPhSerBar1, kPhSerDecide, kPhSerFinal,
+  kPhPair, kNumPhases
+};
 __device__ unsigned long long g_phase_clocks[kNumPhases];
-#define PHASE_MARK(k)                      \
-  do {                                     \
-    if (lane == 0) {                       \
-      const long long now_ = clock64();    \
-      ph_acc[warp][k] += now_ - ph_t;      \
-      ph_t = now_;                         \
-    }                                      \
+// The previous mark's time lives in shared memory and the warp index is read afresh: kept in registers, both would be
+// spilled, and every mark would then wait for a reload from L2 and charge it to the phase it closes.
+#define PHASE_MARK(k)                        \
+  do {                                       \
+    const int ptid_ = fresh_tid();           \
+    if ((ptid_ & 31) == 0) {                 \
+      const long long now_ = clock64();      \
+      ph_acc[ptid_ >> 5][k] += now_ - ph_t[ptid_ >> 5]; \
+      ph_t[ptid_ >> 5] = now_;               \
+    }                                        \
   } while (0)
 #else
 #define PHASE_MARK(k) \
@@ -504,6 +514,15 @@ __device__ __noinline__ void gn_decide(PairCtl* ctl, const double* tot, float ch
   ctl->flag = flag;
 }
 
+// threadIdx.x read afresh from its special register.  Held in a register across the pass loop, the thread index is
+// spilled, and at <128,4> the L1 is almost all shared memory, so every reload is a round trip to L2.  The serial section
+// of a pass tests the thread's role several times on its critical path; each test reads the index here instead.
+__device__ __forceinline__ int fresh_tid() {
+  int t;
+  asm volatile("mov.u32 %0, %%tid.x;" : "=r"(t));
+  return t;
+}
+
 __device__ __forceinline__ void named_barrier_sync(int id, int nthreads) {
   asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
 }
@@ -567,9 +586,11 @@ __global__ void __launch_bounds__(NT, MINB) sparse_img_align_kernel(const AlignA
   uint32_t bar_parity = 0;
 #ifdef PLSVO_PHASE_CLOCKS
   __shared__ unsigned long long ph_acc[NW][kNumPhases];
-  if (lane == 0)
+  __shared__ long long ph_t[NW];
+  if (lane == 0) {
     for (int k = 0; k < kNumPhases; ++k) ph_acc[warp][k] = 0ull;
-  long long ph_t = clock64();
+    ph_t[warp] = clock64();
+  }
 #endif
 
   for (;;) {
@@ -1097,7 +1118,7 @@ __global__ void __launch_bounds__(NT, MINB) sparse_img_align_kernel(const AlignA
         v[29] = (double)n_patch_acc;
         v[30] = 0.0, v[31] = 0.0;
         const double mine = warp_reduce32(v, lane);
-        red[warp * 32 + lane] = mine;
+        red[fresh_tid()] = mine;  // red[warp * 32 + lane]
         __syncthreads();
         PHASE_MARK(kPhReduce);
         if (warp == 0) {
@@ -1106,13 +1127,15 @@ __global__ void __launch_bounds__(NT, MINB) sparse_img_align_kernel(const AlignA
           for (int w = 0; w < NW; ++w) s += red[w * 32 + lane];
           tot[lane] = s;
           __syncwarp();
+          PHASE_MARK(kPhSerRed);
           if (lane == 0) gn_solve(ctl, tot, level);
+          PHASE_MARK(kPhSerSolve);
         }
 #ifdef PLSVO_TREE_CHI2
         if (warp == WALK && lane == 0) ctl->chi2f = 0.f;
         if (false) {
 #else
-        if (warp == WALK) {
+        if ((fresh_tid() >> 5) == WALK) {
 #endif
           // ---- chi2 in the reference's order: chain the composed maps and the opaque patches ----
           float s = 0.f;
@@ -1178,23 +1201,30 @@ __global__ void __launch_bounds__(NT, MINB) sparse_img_align_kernel(const AlignA
             ctl->chi2f = s;  // pt_chi2 (:484); seg_chi2 is added by the decision (:171)
             ctl->n_opq = 0;
           }
+          PHASE_MARK(kPhSerWalk);
         }
-        if (warp == SEGW) {
+        if ((fresh_tid() >> 5) == SEGW) {
           float s2 = 0.f;  // seg_chi2 (:683): one term per accepted segment, in list order (others hold +0, a no-op)
 #pragma unroll 8
           for (int j = 0; j < ns; ++j) s2 = __fadd_rn(s2, seg_term[j]);
           if (lane == 0) ctl->seg_chi2f = s2;
+          PHASE_MARK(kPhSerSegSum);
         }
         // chi2 (walker warp, segment warp) -> decision (thread 0); the warps arrive converged: a named barrier counts
         // whole warps
-        if (NW > 1 && warp * 32 < kSerialThreads) named_barrier_sync(1, kSerialThreads);
+        const int stid = fresh_tid();
+        if (NW > 1 && (stid & ~31) < kSerialThreads) {
+          named_barrier_sync(1, kSerialThreads);
+          PHASE_MARK(kPhSerBar1);
+        }
 #ifdef PLSVO_TREE_CHI2
-        if (tid == 0) gn_decide(ctl, tot, (float)tot[27], a.n_iter, a.eps);
+        if (stid == 0) gn_decide(ctl, tot, (float)tot[27], a.n_iter, a.eps);
 #else
-        if (tid == 0) gn_decide(ctl, tot, __fadd_rn(ctl->chi2f, ctl->seg_chi2f), a.n_iter, a.eps);  // pt_chi2 + seg_chi2 (:171)
+        if (stid == 0) gn_decide(ctl, tot, __fadd_rn(ctl->chi2f, ctl->seg_chi2f), a.n_iter, a.eps);  // pt_chi2 + seg_chi2 (:171)
 #endif
+        PHASE_MARK(kPhSerDecide);
         __syncthreads();
-        PHASE_MARK(kPhSerial);
+        PHASE_MARK(kPhSerFinal);
         if (ctl->flag) break;
       }
     }  // levels
@@ -1311,7 +1341,7 @@ cudaError_t align_kernel_launch(const AlignArgs& a, int grid, int threads, int m
 }  // namespace plsvo
 
 #ifdef PLSVO_PHASE_CLOCKS
-// per-phase cycle sums of sparse_img_align_kernel since the last reset, in the order of the kPh* enum (7 values);
+// per-phase cycle sums of sparse_img_align_kernel since the last reset, in the order of the kPh* enum (13 values);
 // reset != 0 zeroes them afterwards.  Synchronous.  Only in -DPLSVO_PHASE_CLOCKS builds.
 extern "C" int plsvo_phase_clocks(unsigned long long* out, int reset) {
   cudaError_t e = cudaDeviceSynchronize();
