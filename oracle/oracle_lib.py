@@ -583,6 +583,40 @@ def line_seed_update(abi, data, n_threads: int = 1):
     return out
 
 
+SEARCH_STATS_FIELDS = ("steps", "rejected", "level", "first_best", "last_best", "no_win")
+
+
+def seed_search_stats(abi, data, n_threads: int = 1):
+    """The restated point- or line-seed update (by the type of `data`) with a record of every epipolar ZMSSD search ->
+    (abi.SeedOut or abi.LineSeedOut, stats).  stats is a dict of int32 arrays [n] (point seeds) or [n, 2] (line seeds: start
+    point, end point), one per SEARCH_STATS_FIELDS: the step count n_steps + 1 (-1 where no search was reached), whether
+    max_epi_search_steps rejected it, the search level, the first and the last step whose score equals the final best (-1:
+    none), and whether no score beat PatchScore::threshold().  The outputs are those of seed_update / line_seed_update."""
+    lib = load(abi)
+    line = getattr(data, "ref_sf", None) is not None
+    st = np.zeros((data.n, 2 if line else 1, len(SEARCH_STATS_FIELDS)), np.int32)
+    ip = C.POINTER(C.c_int32)
+    if line:
+        fn = lib.plsvo_oracle_line_seed_search_stats
+        fn.argtypes = [C.POINTER(abi.LineSeedBatch), C.POINTER(abi.LineSeedResult), ip, C.c_int]
+        b, keep = abi.make_line_seed_batch(data)
+        out = abi.LineSeedOut(data.n)
+        res = out.line_struct
+    else:
+        fn = lib.plsvo_oracle_seed_search_stats
+        fn.argtypes = [C.POINTER(abi.SeedBatch), C.POINTER(abi.SeedResult), ip, C.c_int]
+        b, keep = abi.make_seed_batch(data)
+        out = abi.SeedOut(data.n)
+        res = out.struct
+    fn.restype = C.c_int
+    rc = fn(C.byref(b), C.byref(res), st.ctypes.data_as(ip), n_threads)
+    if rc != 0:
+        raise RuntimeError(f"oracle seed_search_stats failed rc={rc}")
+    if not line:
+        st = st[:, 0]
+    return out, {k: np.ascontiguousarray(st[..., j]) for j, k in enumerate(SEARCH_STATS_FIELDS)}
+
+
 @_recorded
 def ref_line_seed_update(abi, data):
     """DepthFilter::updateLineSeeds of the reference's own depth_filter.cpp + matcher.cpp -> abi.LineSeedOut (state only)."""

@@ -1633,6 +1633,10 @@ static bool depth_from_triangulation(const SE3& T_search_ref, Vec3 f_ref, Vec3 f
 struct EpiResult {
   int search_level = -1;
   double px_cur[2] = {std::numeric_limits<double>::quiet_NaN(), std::numeric_limits<double>::quiet_NaN()};
+  // statistics of the ZMSSD search (plsvo_oracle_*seed_search_stats; written, never read): its step count n_steps + 1
+  // (-1: the search was never reached), whether max_epi_search_steps rejected it, the first and the last step whose score
+  // equals the final best (-1: none), whether no score beat PatchScore::threshold()
+  int steps = -1, rejected = 0, first_best = -1, last_best = -1, no_win = 0;
 };
 // segment_endpoint = true restates Matcher::findEpipolarMatchDirectSegmentEndpoint (src/matcher.cpp:420-588): NaN depth
 // range and NaN/inf epipolar length are rejected up front, no edgelet pre-selection, otherwise the same search.
@@ -1711,6 +1715,8 @@ static bool find_epipolar_match_direct(const plsvo_seed_batch* in, int i, double
   }
   size_t n_steps = (size_t)(epi_length / 0.7);  // one step per pixel (:345)
   const double step[2] = {epi_dir[0] / (double)n_steps, epi_dir[1] / (double)n_steps};
+  er.steps = n_steps < (size_t)INT32_MAX ? (int)n_steps + 1 : INT32_MAX;
+  er.rejected = n_steps > (size_t)in->max_epi_search_steps;
   if (n_steps > (size_t)in->max_epi_search_steps) return false;
   // ZMSSD of the warped reference patch (:354-356)
   int sumA = 0, sumAA = 0;
@@ -1738,8 +1744,10 @@ static bool find_epipolar_match_direct(const plsvo_seed_batch* in, int i, double
       }
     }
     const int zmssd = sumAA - 2 * sumAB + sumBB - (sumA * sumA - 2 * sumA * sumB + sumB * sumB) / 64;
-    if (zmssd < zmssd_best) zmssd_best = zmssd, uv_best[0] = uv[0], uv_best[1] = uv[1];
+    if (zmssd < zmssd_best) zmssd_best = zmssd, uv_best[0] = uv[0], uv_best[1] = uv[1], er.first_best = (int)k;
+    if (zmssd == zmssd_best && er.first_best >= 0) er.last_best = (int)k;
   }
+  er.no_win = zmssd_best >= 2000 * 64;
   if (zmssd_best < 2000 * 64) {
     er.px_cur[0] = cam.fx * uv_best[0] + cam.cx, er.px_cur[1] = cam.fy * uv_best[1] + cam.cy;
     if (in->subpix_refinement) {
@@ -1797,7 +1805,14 @@ static void update_point_seed(const float x, const float tau2, SeedState* seed) 
   seed->b = seed->a * (1.0f - f) / f;
 }
 
-static void seed_update_one(const plsvo_seed_batch* in, const plsvo_seed_result* out, int i) {
+// one search's record of plsvo_oracle_*seed_search_stats: steps, rejected, search level, first best, last best, no win
+enum { kSearchStats = 6 };
+static void put_search_stats(const EpiResult& er, int32_t* s) {
+  if (!s) return;
+  s[0] = er.steps, s[1] = er.rejected, s[2] = er.search_level, s[3] = er.first_best, s[4] = er.last_best, s[5] = er.no_win;
+}
+
+static void seed_update_one(const plsvo_seed_batch* in, const plsvo_seed_result* out, int i, int32_t* stats = nullptr) {
   const plsvo_camera& cam = in->cam;
   const size_t I = (size_t)i;
   SeedState sd{in->a[i], in->b[i], in->mu[i], in->z_range[i], in->sigma2[i]};
@@ -1840,11 +1855,20 @@ static void seed_update_one(const plsvo_seed_batch* in, const plsvo_seed_result*
     out->converged[i] = (status == PLSVO_SEED_UPDATED && std::sqrt(sd.sigma2) < sd.z_range / in->seed_convergence_sigma2_thresh) ? 1 : 0;
   if (out->depth) out->depth[i] = z;
   if (out->px_cur) out->px_cur[2 * I] = er.px_cur[0], out->px_cur[2 * I + 1] = er.px_cur[1];
+  put_search_stats(er, stats ? stats + kSearchStats * I : nullptr);
 }
 
 int plsvo_oracle_seed_update_batch(const plsvo_seed_batch* in, const plsvo_seed_result* out, int n_threads) {
   if (!in || !out) return PLSVO_ERR_INVALID;
   parallel_for(in->n_seeds, n_threads, [&](int i) { seed_update_one(in, out, i); });
+  return PLSVO_OK;
+}
+
+// The same update, also recording the epipolar search of every seed: stats [n_seeds][kSearchStats] (test infrastructure:
+// which step counts, ties and winners a test batch exercises).
+int plsvo_oracle_seed_search_stats(const plsvo_seed_batch* in, const plsvo_seed_result* out, int32_t* stats, int n_threads) {
+  if (!in || !out || !stats) return PLSVO_ERR_INVALID;
+  parallel_for(in->n_seeds, n_threads, [&](int i) { seed_update_one(in, out, i, stats); });
   return PLSVO_OK;
 }
 
@@ -1875,7 +1899,7 @@ static void line_endpoint_update(float x, float tau2, float norm_scale, float a,
   mu = mu_new;
 }
 
-static void line_seed_update_one(const plsvo_line_seed_batch* inl, const plsvo_line_seed_result* outl, int i) {
+static void line_seed_update_one(const plsvo_line_seed_batch* inl, const plsvo_line_seed_result* outl, int i, int32_t* stats = nullptr) {
   const plsvo_seed_batch* in = &inl->seeds;
   const plsvo_seed_result* out = &outl->seeds;
   const plsvo_camera& cam = in->cam;
@@ -1943,11 +1967,21 @@ static void line_seed_update_one(const plsvo_line_seed_batch* inl, const plsvo_l
   if (outl->depth_e) outl->depth_e[i] = z_e;
   if (out->px_cur) out->px_cur[2 * I] = er_s.px_cur[0], out->px_cur[2 * I + 1] = er_s.px_cur[1];
   if (outl->px_cur_e) outl->px_cur_e[2 * I] = er_e.px_cur[0], outl->px_cur_e[2 * I + 1] = er_e.px_cur[1];
+  put_search_stats(er_s, stats ? stats + kSearchStats * 2 * I : nullptr);
+  put_search_stats(er_e, stats ? stats + kSearchStats * (2 * I + 1) : nullptr);
 }
 
 int plsvo_oracle_line_seed_update_batch(const plsvo_line_seed_batch* in, const plsvo_line_seed_result* out, int n_threads) {
   if (!in || !out) return PLSVO_ERR_INVALID;
   parallel_for(in->seeds.n_seeds, n_threads, [&](int i) { line_seed_update_one(in, out, i); });
+  return PLSVO_OK;
+}
+
+// plsvo_oracle_seed_search_stats for line seeds: stats [n_seeds][2][kSearchStats], start point then end point (an end point
+// whose start point did not match is never searched)
+int plsvo_oracle_line_seed_search_stats(const plsvo_line_seed_batch* in, const plsvo_line_seed_result* out, int32_t* stats, int n_threads) {
+  if (!in || !out || !stats) return PLSVO_ERR_INVALID;
+  parallel_for(in->seeds.n_seeds, n_threads, [&](int i) { line_seed_update_one(in, out, i, stats); });
   return PLSVO_OK;
 }
 

@@ -933,7 +933,7 @@ cudaError_t match_direct_kernel_launch(const MatchArgs& a, cudaStream_t s) {
   return cudaGetLastError();
 }
 
-// seeds per warp: as many as keeps ~8 warps on every SM (a power of two between 1 and 32); PLSVO_SEEDS_PER_WARP overrides
+// seeds per warp: as many as keeps ~8 warps on every SM (a power of two between 1 and 32)
 static int seeds_per_warp(int n) {
   static int sms = 0;
   if (sms == 0) {
@@ -944,27 +944,23 @@ static int seeds_per_warp(int n) {
   }
   int spw = 1;
   while (spw < 32 && (long long)n > (long long)spw * sms * 8) spw <<= 1;
-  if (const char* e = getenv("PLSVO_SEEDS_PER_WARP")) {
-    const int v = atoi(e);
-    if (v >= 1 && v <= 32) spw = v;
-  }
   return spw;
 }
 // steps of a search its own thread walks before the warp takes over: worth it only when most lanes hold a seed
-static int own_thread_steps(int spw) {
-  int t = spw >= 16 ? 16 : 0;
-  if (const char* e = getenv("PLSVO_EPI_SERIAL_STEPS")) {
-    const int v = atoi(e);
-    if (v >= 0 && v <= 100000) t = v;
-  }
-  return t;
+static int own_thread_steps(int spw) { return spw >= 16 ? 16 : 0; }
+
+// the schedule of a launch: the caller's forced values (PLSVO_SEEDS_PER_WARP / PLSVO_EPI_SERIAL_STEPS, validated by the host
+// code) where set, the automatic choice elsewhere
+static SeedArgs seed_schedule(const SeedArgs& a0) {
+  SeedArgs a = a0;
+  if (a.spw < 1) a.spw = seeds_per_warp(a.n);
+  if (a.serial_steps < 0) a.serial_steps = own_thread_steps(a.spw);
+  return a;
 }
 
 cudaError_t line_seed_update_kernel_launch(const SeedArgs& a0, cudaStream_t s) {
   if (a0.n <= 0) return cudaSuccess;
-  SeedArgs a = a0;
-  a.spw = seeds_per_warp(a.n);
-  a.serial_steps = own_thread_steps(a.spw);
+  const SeedArgs a = seed_schedule(a0);
   const int per_cta = a.spw * (kA2Threads / 32);
   line_seed_update_kernel<<<(a.n + per_cta - 1) / per_cta, kA2Threads, 0, s>>>(a);
   return cudaGetLastError();
@@ -972,9 +968,7 @@ cudaError_t line_seed_update_kernel_launch(const SeedArgs& a0, cudaStream_t s) {
 
 cudaError_t seed_update_kernel_launch(const SeedArgs& a0, cudaStream_t s) {
   if (a0.n <= 0) return cudaSuccess;
-  SeedArgs a = a0;
-  a.spw = seeds_per_warp(a.n);
-  a.serial_steps = own_thread_steps(a.spw);
+  const SeedArgs a = seed_schedule(a0);
   const int per_cta = a.spw * (kA2Threads / 32);
   seed_update_kernel<<<(a.n + per_cta - 1) / per_cta, kA2Threads, 0, s>>>(a);
   return cudaGetLastError();

@@ -219,8 +219,8 @@ cudaError_t match_direct_kernel_launch(const MatchArgs& a, cudaStream_t s);
 // ---------------------------------------------------------------------------------------------
 struct SeedArgs {
   int n, n_iter, n_pyr_levels, width, height, max_epi_search_steps;
-  int spw;           // seeds per warp (set by the launch functions)
-  int serial_steps;  // steps of an epipolar search walked by the seed's own thread before the warp takes over
+  int spw;           // seeds per warp; -1: chosen by the launch functions from the batch size
+  int serial_steps;  // steps of an epipolar search walked by the seed's own thread before the warp takes over; -1: automatic
   int align_1d, subpix_refinement, edgelet_filtering;
   double edgelet_max_angle, convergence_thresh;
   double fx, fy, cx, cy;

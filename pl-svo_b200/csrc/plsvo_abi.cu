@@ -2,6 +2,7 @@
 // Host-side only; the kernels are in align_kernel.cu and poseopt_kernel.cu.
 #include <cuda_runtime.h>
 #include <chrono>
+#include <errno.h>
 #include <math.h>
 #include <stdio.h>
 #include <stdlib.h>
@@ -1530,12 +1531,35 @@ static int structopt_batch_run_body(plsvo_ctx* ctx, const plsvo_structopt_batch*
 }
 
 namespace {
+// PLSVO_SEEDS_PER_WARP and PLSVO_EPI_SERIAL_STEPS force the search schedule of the seed kernels (tests, A/B runs).  Unset
+// or empty means automatic (*v = -1).  Any other value must be a whole number in [lo, hi]: a switch that is set but not
+// honoured would leave whoever set it measuring the automatic schedule without knowing.
+int schedule_override(plsvo_ctx_impl* c, const char* name, int lo, int hi, int* v) {
+  *v = -1;
+  const char* e = getenv(name);
+  if (!e || !*e) return PLSVO_OK;
+  char* end = nullptr;
+  errno = 0;
+  const long x = strtol(e, &end, 10);
+  if (end == e || *end || errno || x < lo || x > hi) {
+    char msg[160];
+    snprintf(msg, sizeof msg, "%s=\"%.40s\" is not a whole number in [%d, %d]", name, e, lo, hi);
+    return fail(c, PLSVO_ERR_INVALID, msg);
+  }
+  *v = (int)x;
+  return PLSVO_OK;
+}
+
 // point seeds (lin == nullptr) and line seeds share staging; the line variant adds the end-point arrays
 int seed_update_run(plsvo_ctx_impl* c, const plsvo_seed_batch* in, const plsvo_seed_result* out, const plsvo_line_seed_batch* lin,
                     const plsvo_line_seed_result* lout) {
   if (in->n_seeds < 0 || in->n_ref_images <= 0 || in->n_cur_images <= 0 || in->cam.width <= 0 || in->cam.height <= 0 ||
       in->n_iter < 0 || in->n_pyr_levels < 1 || in->n_pyr_levels > PLSVO_MAX_LEVELS || in->max_epi_search_steps < 0)
     return fail(c, PLSVO_ERR_INVALID, "seed batch description");
+  int spw = -1, serial_steps = -1;
+  int rc = schedule_override(c, "PLSVO_SEEDS_PER_WARP", 1, 32, &spw);
+  if (rc == PLSVO_OK) rc = schedule_override(c, "PLSVO_EPI_SERIAL_STEPS", 0, 100000, &serial_steps);
+  if (rc != PLSVO_OK) return rc;
   if (in->n_seeds == 0) return PLSVO_OK;
   if (!in->T_ref_w || !in->T_cur_w || !in->ref_index || !in->cur_index || !in->ref_px || !in->ref_f || !in->ref_level || !in->a ||
       !in->b || !in->mu || !in->z_range || !in->sigma2 || !out->a || !out->b || !out->mu || !out->sigma2 || !out->status)
@@ -1560,11 +1584,12 @@ int seed_update_run(plsvo_ctx_impl* c, const plsvo_seed_batch* in, const plsvo_s
   SeedArgs a;
   memset(&a, 0, sizeof a);
   a.n = in->n_seeds, a.n_iter = in->n_iter, a.n_pyr_levels = in->n_pyr_levels, a.max_epi_search_steps = in->max_epi_search_steps;
+  a.spw = spw, a.serial_steps = serial_steps;
   a.align_1d = in->align_1d, a.subpix_refinement = in->subpix_refinement, a.edgelet_filtering = in->epi_search_edgelet_filtering;
   a.edgelet_max_angle = in->epi_search_edgelet_max_angle, a.convergence_thresh = in->seed_convergence_sigma2_thresh;
   a.width = in->cam.width, a.height = in->cam.height;
   a.fx = in->cam.fx, a.fy = in->cam.fy, a.cx = in->cam.cx, a.cy = in->cam.cy;
-  int rc = stage_pyramid(c, c->m_ref_img, in->ref_img, in->ref_pitch, in->ref_stride, in->n_ref_images, a.width, a.height, s, a.ref_img,
+  rc = stage_pyramid(c, c->m_ref_img, in->ref_img, in->ref_pitch, in->ref_stride, in->n_ref_images, a.width, a.height, s, a.ref_img,
                          a.ref_pitch, a.ref_stride);
   if (rc != PLSVO_OK) return rc;
   rc = stage_pyramid(c, c->m_cur_img, in->cur_img, in->cur_pitch, in->cur_stride, in->n_cur_images, a.width, a.height, s, a.cur_img,

@@ -35,6 +35,7 @@ class Camera:
 VGA = Camera(640, 480, 420.0, 420.0, 319.5, 239.5)
 HD720 = Camera(1280, 720, 840.0, 840.0, 639.5, 359.5)
 QVGA = Camera(320, 240, 210.0, 210.0, 159.5, 119.5)  # small case for fast CPU tests
+ODD = Camera(641, 479, 420.0, 420.0, 320.0, 239.0)  # odd sizes: no level is a multiple of 16 pixels wide
 
 
 # ------------------------------------------------------------------------------------------------

@@ -404,6 +404,34 @@ def s_forced_variant_is_the_only_one_tried():
     clean()
 
 
+def s_seed_schedule_overrides_are_validated():
+    """PLSVO_SEEDS_PER_WARP (1 ... 32) and PLSVO_EPI_SERIAL_STEPS (0 ... 100000) force the search schedule of the seed
+    kernels: any other value fails the call before anything is queued and names the variable; empty means automatic."""
+    ctx = pkg.api.Context(0)
+    pts = synth.make_seed_batch(cam=synth.QVGA, n=40, seed=9990)
+    lines = synth.make_line_seed_batch(cam=synth.QVGA, n=40, seed=9991)
+    bp, keep_p = abi.make_seed_batch(pts)
+    bl, keep_l = abi.make_line_seed_batch(lines)
+    op, ol = abi.SeedOut(pts.n), abi.LineSeedOut(lines.n)
+    calls = (lambda: ctx.lib.plsvo_seed_update_batch_run(ctx.handle, C.byref(bp), C.byref(op.struct)),
+             lambda: ctx.lib.plsvo_line_seed_update_batch_run(ctx.handle, C.byref(bl), C.byref(ol.line_struct)))
+    cases = {"PLSVO_SEEDS_PER_WARP": (("0", "33", "-1", "8x", "x", " ", "4.5", "99999999999"), ("1", "3", "32", "")),
+             "PLSVO_EPI_SERIAL_STEPS": (("-1", "100001", "16 ", "abc", "1e3"), ("0", "17", "100000", ""))}
+    for var, (bad, good) in cases.items():
+        for v in bad + good:
+            for call in calls:
+                with env(**{var: v}):
+                    rc = call()
+                msg = (ctx.lib.plsvo_last_error(ctx.handle) or b"").decode()
+                if v in bad:
+                    assert rc == abi.ERR_INVALID and var in msg, f"{var}={v!r}: rc {rc}, {msg!r}"
+                    assert lib.fake_cuda_pending_ops() == 0, f"{var}={v!r}: work queued by a rejected call"
+                else:  # accepted: the call reaches the kernel, which this model (no oracle behind it) does not answer
+                    assert rc != abi.ERR_INVALID and var not in msg, f"{var}={v!r}: rc {rc}, {msg!r}"
+                lib.fake_cuda_clear_errors()
+                clean()
+
+
 def poseopt_expected(po, T=None):
     B = po.batch
     want = np.zeros(B, np.uint64)

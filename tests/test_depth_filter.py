@@ -10,7 +10,8 @@ import pytest
 
 
 @pytest.mark.parametrize("seed,kw", [(9000, {}), (9001, dict(n_pyr_levels=5)), (9002, dict(baseline=0.3)),
-                                     (9003, dict(cam="QVGA")), (9004, dict(edgelet_frac=0.8))])
+                                     (9003, dict(cam="QVGA")), (9004, dict(edgelet_frac=0.8)),
+                                     (9005, dict(cam="EUROC", n_pyr_levels=5)), (9006, dict(cam="ODD", n_pyr_levels=5))])
 def test_oracle_seed_update_is_bit_identical_to_the_reference_tus(oracle, abi, synth, seed, kw):
     if not oracle.have_ref():
         pytest.skip("oracle/_ref is not built and no recorded outputs of it are present")
@@ -58,8 +59,12 @@ def test_oracle_seed_update_measures_depth_and_shrinks_the_variance(oracle, abi,
 
 
 @pytest.mark.gpu
-@pytest.mark.parametrize("seed,kw", [(9100, {}), (9101, dict(n_pyr_levels=5, baseline=0.25)), (9102, dict(edgelet_frac=0.6))])
+@pytest.mark.parametrize("seed,kw", [(9100, {}), (9101, dict(n_pyr_levels=5, baseline=0.25)), (9102, dict(edgelet_frac=0.6)),
+                                     (9103, dict(cam="EUROC", n_pyr_levels=5)), (9104, dict(cam="ODD", n_pyr_levels=5))])
 def test_gpu_seed_update_matches_the_oracle(pkg, oracle, abi, synth, gen_device, seed, kw):
+    kw = dict(kw)
+    if "cam" in kw:
+        kw["cam"] = getattr(synth, kw["cam"])
     d = synth.make_seed_batch(n=6000, seed=seed, device=gen_device, **kw)
     ref = oracle.seed_update(abi, d, 8)
     out = pkg.DepthFilter().updatePointSeeds(d)
@@ -110,7 +115,8 @@ def test_gpu_seed_update_options_and_bad_input(pkg, oracle, abi, synth, gen_devi
 LINE_FIELDS = ("a", "b", "mu", "sigma2", "mu_e", "sigma2_e")
 
 
-@pytest.mark.parametrize("seed,kw", [(9500, {}), (9501, dict(n_pyr_levels=5)), (9502, dict(baseline=0.3)), (9503, dict(cam="QVGA"))])
+@pytest.mark.parametrize("seed,kw", [(9500, {}), (9501, dict(n_pyr_levels=5)), (9502, dict(baseline=0.3)), (9503, dict(cam="QVGA")),
+                                     (9504, dict(cam="EUROC", n_pyr_levels=5)), (9505, dict(cam="ODD", n_pyr_levels=5))])
 def test_oracle_line_seed_update_is_bit_identical_to_the_reference_tus(oracle, abi, synth, seed, kw):
     if not oracle.have_ref():
         pytest.skip("oracle/_ref is not built and no recorded outputs of it are present")

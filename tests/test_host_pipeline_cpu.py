@@ -31,7 +31,7 @@ ABI_SOURCE = os.path.join(os.path.dirname(HERE), "pl-svo_b200", "csrc", "plsvo_a
 SCENARIOS = ["plain_upload_launch_download", "small_batch_staging_block", "staging_block_grows_while_a_copy_is_queued", "three_leg_api_and_relaunch",
              "arrival_gated_stream", "padded_host_layouts", "lean_features", "chain_every_host_path", "chain_arrival_gated_stream",
              "chain_padded_host_layouts", "rejected_inputs_leave_nothing_in_flight", "forced_variant_is_the_only_one_tried",
-             "pose_optimiser_host_paths", "pyramid_call",
+             "seed_schedule_overrides_are_validated", "pose_optimiser_host_paths", "pyramid_call",
              "track_chained_call", "randomised_configurations", "bench_chain_leg"]
 
 

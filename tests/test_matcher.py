@@ -5,7 +5,8 @@ import numpy as np
 import pytest
 
 
-@pytest.mark.parametrize("seed,levels,cam", [(7000, 3, "VGA"), (7001, 5, "VGA"), (7002, 3, "QVGA"), (7003, 4, "HD720")])
+@pytest.mark.parametrize("seed,levels,cam", [(7000, 3, "VGA"), (7001, 5, "VGA"), (7002, 3, "QVGA"), (7003, 4, "HD720"), (7004, 5, "EUROC"),
+                                             (7005, 5, "ODD")])
 def test_oracle_find_match_direct_is_bit_identical_to_the_reference_tu(oracle, abi, synth, seed, levels, cam):
     if not oracle.have_ref():
         pytest.skip("oracle/_ref is not built and no recorded outputs of it are present")
@@ -35,7 +36,7 @@ def test_oracle_find_match_direct_refines_towards_the_true_projection(oracle, ab
 
 
 @pytest.mark.gpu
-@pytest.mark.parametrize("seed,levels,cam", [(7100, 3, "VGA"), (7101, 5, "VGA"), (7102, 4, "HD720")])
+@pytest.mark.parametrize("seed,levels,cam", [(7100, 3, "VGA"), (7101, 5, "VGA"), (7102, 4, "HD720"), (7103, 5, "EUROC"), (7104, 5, "ODD")])
 def test_gpu_find_match_direct_is_bit_identical_to_the_oracle(pkg, oracle, abi, synth, gen_device, seed, levels, cam):
     d = synth.make_match_batch(cam=getattr(synth, cam), n=6000, seed=seed, n_pyr_levels=levels, device=gen_device)
     ref = oracle.match_direct(abi, d, 8)
