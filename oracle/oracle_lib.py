@@ -97,6 +97,44 @@ def poseopt(abi, data, params=None, n_threads: int = 1):
     return out
 
 
+# exit reasons of a Gauss-Newton loop in poseopt_stats
+PO_EXIT_NONE, PO_EXIT_CHI2, PO_EXIT_NAN, PO_EXIT_EPS, PO_EXIT_CAP = range(5)
+PO_MEDIANS = ("mad_pt", "mad_ls", "init", "final")
+PO_STAT_ITERS = 32
+
+
+def poseopt_stats(abi, data, params=None, n_threads: int = 1):
+    """The restated pose optimiser with a record of every frame's decisions -> (abi.PoseOptOut, stats).  The outputs are
+    those of poseopt.  stats is a dict of arrays over the batch; [.., 2] is (main loop, refinement loop):
+      exit [B,2]            PO_EXIT_*: chi2 rise, NaN step, EPS, iteration cap, or no iteration (also: no observation)
+      fallback [B,2]        some solve's A has an unpivoted LDL^T pivot not above 1e-13 * max|diag A| (the GPU's register
+                            solve then hands the system to the pivoted one)
+      scale_pt, scale_ls [B]  the two MAD scales, before the fx factor
+      med_count, med_tie [B,4]  per PO_MEDIANS: the live count, and whether the key of rank n // 2 is tied with a neighbour
+      out_margin_pt, out_margin_ls [B]  smallest |e - thr| / thr of the outlier decisions (inf: none, or thr infinite)
+      chi2_margin, eps_margin [B,2]  smallest relative margin of the new_chi2 > chi2 and norm_max(dT) <= EPS decisions
+      iter_margin [B,2,PO_STAT_ITERS]  the smaller of the two at each iteration (inf: no such decision)"""
+    lib = load(abi)
+    params = params or abi.poseopt_params()
+    batch, keep = abi.make_poseopt_batch(data)
+    out = abi.PoseOptOut(data.batch, data.n_pts, data.n_segs)
+    lib.plsvo_oracle_poseopt_stats_stride.restype = C.c_int
+    stride = lib.plsvo_oracle_poseopt_stats_stride()
+    assert stride == 20 + 2 * PO_STAT_ITERS
+    st = np.zeros((data.batch, stride))
+    fn = lib.plsvo_oracle_poseopt_stats
+    fn.restype = C.c_int
+    fn.argtypes = [C.POINTER(abi.PoseOptBatch), C.POINTER(abi.PoseOptParams), C.POINTER(abi.PoseOptResult), C.POINTER(C.c_double), C.c_int]
+    rc = fn(C.byref(batch), C.byref(params), C.byref(out.struct), st.ctypes.data_as(C.POINTER(C.c_double)), n_threads)
+    if rc != 0:
+        raise RuntimeError(f"oracle poseopt_stats failed rc={rc}")
+    return out, {
+        "exit": st[:, 0:2].astype(np.int32), "fallback": st[:, 2:4] != 0, "scale_pt": st[:, 4].copy(), "scale_ls": st[:, 5].copy(),
+        "med_count": st[:, 6:10].astype(np.int64), "med_tie": st[:, 10:14] != 0, "out_margin_pt": st[:, 14].copy(),
+        "out_margin_ls": st[:, 15].copy(), "chi2_margin": st[:, 16:18].copy(), "eps_margin": st[:, 18:20].copy(),
+        "iter_margin": st[:, 20:].reshape(-1, 2, PO_STAT_ITERS).copy()}
+
+
 def pyramid(abi, img0, n_levels: int):
     """frame_utils::createImgPyramid restated: u8 [B,H,W] -> list of levels."""
     lib = load(abi)

@@ -842,7 +842,68 @@ inline void project2d(Vec3 p, double uv[2]) {  // vk::project2d
   uv[1] = p.y / p.z;
 }
 
-void poseopt_one(const plsvo_poseopt_batch* B, const plsvo_poseopt_params* P, const plsvo_poseopt_result* out, int b) {
+// One frame's record of plsvo_oracle_poseopt_stats (doubles), per loop l (0 main, 1 refinement) where marked [2]:
+//   exit[2]           why the loop ended: kPoExit*
+//   fallback[2]       1 if some solve's A has an unpivoted LDL^T pivot that is not > 1e-13 * max|diag A|
+//   scale_pt, scale_ls  the two MAD scales (before the fx factor)
+//   med_count[4], med_tie[4]  the MAD point, MAD segment, error_init and error_final medians: live count, and whether
+//                     the key of rank floor(n/2) equals a neighbour in sorted order
+//   out_margin_pt, out_margin_ls  smallest |e - thr| / thr of the outlier decisions (inf: none, or an infinite thr)
+//   chi2_margin[2]    smallest |new_chi2 - chi2| / max(|new_chi2|, |chi2|) of the new_chi2 > chi2 decisions evaluated
+//   eps_margin[2]     smallest |norm_max(dT) - EPS| / EPS of the convergence decisions evaluated
+//   iter_margin[2][kPoStatIters]  the smaller of the two at each iteration (inf: no decision with a margin)
+enum { kPoExitNone = 0, kPoExitChi2 = 1, kPoExitNan = 2, kPoExitEps = 3, kPoExitCap = 4 };
+enum {
+  kPoStatIters = 32,
+  kPoSExit = 0, kPoSFallback = 2, kPoSScalePt = 4, kPoSScaleLs = 5, kPoSMedCount = 6, kPoSMedTie = 10, kPoSOutPt = 14,
+  kPoSOutLs = 15, kPoSChi2 = 16, kPoSEps = 18, kPoSIter = 20, kPoStats = kPoSIter + 2 * kPoStatIters
+};
+inline void keep_min(double& slot, double m) {  // a NaN margin sticks
+  if (std::isnan(slot)) return;
+  if (std::isnan(m) || m < slot) slot = m;
+}
+inline double outlier_margin(double e, double thr) {  // an infinite threshold keeps every feature, whatever round-off
+  return std::isinf(thr) ? std::numeric_limits<double>::infinity() : std::fabs(e - thr) / thr;
+}
+inline double rel_margin(double a, double b) {
+  const double s = std::max(std::fabs(a), std::fabs(b));
+  return s > 0.0 ? std::fabs(a - b) / s : 0.0;
+}
+// The register solve's acceptance rule, from its statement rather than its code: without pivoting, A = L D L^T must
+// have every d_j = A_jj - sum_{k<j} L_jk^2 d_k above 1e-13 times the largest |A_ii|; otherwise the pivoted solve runs.
+inline bool reg_rule_rejects(const double A[36]) {
+  double dmax = 0.0;
+  for (int i = 0; i < 6; ++i) dmax = std::max(dmax, std::fabs(A[i * 6 + i]));
+  double L[6][6] = {}, d[6];
+  for (int j = 0; j < 6; ++j) {
+    double s = A[j * 6 + j];
+    for (int k = 0; k < j; ++k) s -= L[j][k] * L[j][k] * d[k];
+    if (!(s > 1e-13 * dmax)) return true;
+    d[j] = s;
+    for (int i = j + 1; i < 6; ++i) {
+      double t = A[i * 6 + j];
+      for (int k = 0; k < j; ++k) t -= L[i][k] * L[j][k] * d[k];
+      L[i][j] = t / s;
+    }
+  }
+  return false;
+}
+template <class T>
+void median_stats(std::vector<T> v, double* st, int which) {  // on a copy: get_median reorders its argument
+  const size_t n = v.size(), k = n / 2;
+  st[kPoSMedCount + which] = (double)n;
+  if (n == 0) return;
+  std::sort(v.begin(), v.end());
+  st[kPoSMedTie + which] = ((k > 0 && v[k - 1] == v[k]) || (k + 1 < n && v[k + 1] == v[k])) ? 1.0 : 0.0;
+}
+
+void poseopt_one(const plsvo_poseopt_batch* B, const plsvo_poseopt_params* P, const plsvo_poseopt_result* out, int b,
+                 double* st = nullptr) {
+  if (st) {
+    const double inf = std::numeric_limits<double>::infinity();
+    std::fill(st, st + kPoStats, 0.0);
+    std::fill(st + kPoSOutPt, st + kPoStats, inf);  // every margin
+  }
   const int np = B->pt_count ? B->pt_count[b] : B->n_pts;
   const int ns = B->seg_count ? B->seg_count[b] : B->n_segs;
   const size_t po = (size_t)b * B->n_pts, so = (size_t)b * B->n_segs;
@@ -886,6 +947,7 @@ void poseopt_one(const plsvo_poseopt_batch* B, const plsvo_poseopt_params* P, co
   }
   // NOTE: the reference calls getMedian on an empty vector (UB) when there are no valid points but
   // there are lines; we define that case as scale 0 (the assert in vk::getMedian would fire).
+  if (st) median_stats(errors, st, 0);
   double estimated_scale_pt = errors.empty() ? 0.0 : (double)mad_scale(errors);
   size_t num_obs_pt = errors.size();
   // :73-87
@@ -909,12 +971,19 @@ void poseopt_one(const plsvo_poseopt_batch* B, const plsvo_poseopt_params* P, co
   if (out->status) out->status[b] = 0;
   size_t num_obs_ls = errors_ls.size();
   double estimated_scale_ls = 1.f;
+  if (st) median_stats(errors_ls, st, 1);
   if (!errors_ls.empty()) estimated_scale_ls = mad_scale(errors_ls);
   double estimated_scale = estimated_scale_pt;
   const double scale_pt = estimated_scale_pt, scale_ls = estimated_scale_ls;
+  if (st) st[kPoSScalePt] = scale_pt, st[kPoSScaleLs] = scale_ls;
 
   // one GN loop (:103-195 and, for the 10-arg overload, :473-563)
   auto gn_loop = [&](size_t n_iter, int which) {
+    if (st) st[kPoSExit + which] = n_iter > 0 ? kPoExitCap : kPoExitNone;
+    auto margin = [&](size_t iter, int slot, double m) {
+      keep_min(st[slot + which], m);
+      if (iter < (size_t)kPoStatIters) keep_min(st[kPoSIter + which * kPoStatIters + iter], m);
+    };
     for (size_t iter = 0; iter < n_iter; iter++) {
       std::fill(A, A + 36, 0.0);
       std::fill(bvec, bvec + 6, 0.0);
@@ -978,7 +1047,12 @@ void poseopt_one(const plsvo_poseopt_batch* B, const plsvo_poseopt_params* P, co
       double dT[6];
       solve6(A, bvec, dT);
       if (out->iters) out->iters[2 * (size_t)b + which] += 1;
+      if (st) {
+        if (reg_rule_rejects(A)) st[kPoSFallback + which] = 1.0;
+        if (iter > 0) margin(iter, kPoSChi2, rel_margin(new_chi2, chi2));
+      }
       if ((iter > 0 && new_chi2 > chi2) || std::isnan(dT[0])) {
+        if (st) st[kPoSExit + which] = (iter > 0 && new_chi2 > chi2) ? kPoExitChi2 : kPoExitNan;
         T = T_old;
         break;
       }
@@ -986,7 +1060,11 @@ void poseopt_one(const plsvo_poseopt_batch* B, const plsvo_poseopt_params* P, co
       T_old = T;
       T = T_new;
       chi2 = new_chi2;
-      if (norm_max6(dT) <= 0.0000000001) break;  // EPS, global.h:99
+      if (st) margin(iter, kPoSEps, std::fabs(norm_max6(dT) - 0.0000000001) / 0.0000000001);
+      if (norm_max6(dT) <= 0.0000000001) {  // EPS, global.h:99
+        if (st) st[kPoSExit + which] = kPoExitEps;
+        break;
+      }
     }
   };
 
@@ -1012,6 +1090,7 @@ void poseopt_one(const plsvo_poseopt_batch* B, const plsvo_poseopt_params* P, co
     e[0] *= s, e[1] *= s;
     const double e_sq = e[0] * e[0] + e[1] * e[1];
     chi2_vec_final.push_back(e_sq);
+    if (st) keep_min(st[kPoSOutPt], outlier_margin(std::sqrt(e_sq), reproj_thresh_scaled_pt));
     if (std::sqrt(e_sq) > reproj_thresh_scaled_pt) {
       pt_alive[i] = 0;
       ++n_deleted_refs_pt;
@@ -1028,6 +1107,7 @@ void poseopt_one(const plsvo_poseopt_batch* B, const plsvo_poseopt_params* P, co
     e[0] *= s, e[1] *= s;
     const double e_sq = e[0] * e[0] + e[1] * e[1];
     chi2_vec_final.push_back(e_sq);
+    if (st) keep_min(st[kPoSOutLs], outlier_margin(std::sqrt(e_sq), reproj_thresh_scaled_ls));
     if (std::sqrt(e_sq) > reproj_thresh_scaled_ls) {
       seg_alive[j] = 0;
       ++n_deleted_refs_ls;
@@ -1036,6 +1116,7 @@ void poseopt_one(const plsvo_poseopt_batch* B, const plsvo_poseopt_params* P, co
 
   if (P->n_iter_ref >= 0) gn_loop((size_t)P->n_iter_ref, 1);  // :469-563 refinement with inliers
 
+  if (st) median_stats(chi2_vec_init, st, 2), median_stats(chi2_vec_final, st, 3);
   double error_init = 0.0, error_final = 0.0;
   if (!chi2_vec_init.empty()) error_init = std::sqrt(get_median(chi2_vec_init)) * fx;
   if (!chi2_vec_final.empty()) error_final = std::sqrt(get_median(chi2_vec_final)) * fx;
@@ -1105,6 +1186,16 @@ int plsvo_oracle_poseopt_batch(const plsvo_poseopt_batch* batch, const plsvo_pos
                                const plsvo_poseopt_result* out, int n_threads) {
   if (!batch || !params || !out) return PLSVO_ERR_INVALID;
   parallel_for(batch->batch, n_threads, [&](int b) { poseopt_one(batch, params, out, b); });
+  return PLSVO_OK;
+}
+
+// The same optimisation, also recording every frame's decisions: stats [batch][plsvo_oracle_poseopt_stats_stride()]
+// doubles, laid out as described at poseopt_one (test infrastructure: which exits, ties and near-ties a test batch reaches).
+int plsvo_oracle_poseopt_stats_stride(void) { return kPoStats; }
+int plsvo_oracle_poseopt_stats(const plsvo_poseopt_batch* batch, const plsvo_poseopt_params* params,
+                               const plsvo_poseopt_result* out, double* stats, int n_threads) {
+  if (!batch || !params || !out || !stats) return PLSVO_ERR_INVALID;
+  parallel_for(batch->batch, n_threads, [&](int b) { poseopt_one(batch, params, out, b, stats + (size_t)kPoStats * b); });
   return PLSVO_OK;
 }
 

@@ -415,9 +415,10 @@ def make_poseopt_batch(
     pert_r: float = 0.01,
     scene: Scene | None = None,
     T_gt: np.ndarray | None = None,
+    max_level: int = 2,
 ) -> PoseOptData:
     """B frames; observations = GT projection + N(0,(noise_px/fx)^2) on the unit plane, 10 % outliers
-    (U[5,30] px), level in {0,1,2}; initial pose = exp(delta) * T_gt.  T_gt [B,7]: ground-truth poses to use (the
+    (U[5,30] px), level in {0, ..., max_level}; initial pose = exp(delta) * T_gt.  T_gt [B,7]: ground-truth poses to use (the
     chained align -> pose-opt case observes the features in the alignment's current frame)."""
     scene = scene or Scene()
     rng = np.random.Generator(np.random.PCG64(seed))
@@ -453,7 +454,7 @@ def make_poseopt_batch(
     uv = perturb(d, n_pts)
     f = torch.cat([uv, torch.ones_like(uv[..., :1])], -1)
     pt_f = f / f.norm(dim=-1, keepdim=True)
-    pt_level = rng.integers(0, 3, (batch, n_pts)).astype(np.int32)
+    pt_level = rng.integers(0, max_level + 1, (batch, n_pts)).astype(np.int32)
 
     spx = np.stack([rng.uniform(m, cam.width - m, (batch, n_segs)), rng.uniform(m, cam.height - m, (batch, n_segs))], -1)
     epx = np.stack([rng.uniform(m, cam.width - m, (batch, n_segs)), rng.uniform(m, cam.height - m, (batch, n_segs))], -1)
@@ -467,7 +468,7 @@ def make_poseopt_batch(
     ef = ef / ef.norm(dim=-1, keepdim=True)
     line = torch.linalg.cross(sf, ef)  # src/feature.cpp:93-107
     line = line / torch.sqrt(line[..., 0:1] ** 2 + line[..., 1:2] ** 2)
-    seg_level = rng.integers(0, 3, (batch, n_segs)).astype(np.int32)
+    seg_level = rng.integers(0, max_level + 1, (batch, n_segs)).astype(np.int32)
 
     npy = lambda t: np.ascontiguousarray(t.detach().cpu().numpy())
     return PoseOptData(
