@@ -169,6 +169,111 @@ def align2d(abi, cur_pyr, image_index, level, border, ref, px, n_iter):
     return conv, out
 
 
+# ---- align2D / align1D / findMatchDirect over whole batches, on all cores, optionally with each feature's decisions --------
+# The record of one feature (plsvo_oracle_direct_stats_stride() doubles, laid out at DirectStats in plsvo_oracle.cpp)
+DS_EXIT_NONE, DS_EXIT_FRAME, DS_EXIT_CONVERGED, DS_EXIT_CAP, DS_EXIT_BACKOFF = range(5)
+DS_BOUNDS = ("left", "top", "right", "bottom")  # the order of stats["dist"] columns and of the stats["bound"] bits
+
+
+def _n_threads(abi, n_threads):
+    return n_threads or max(1, load(abi).plsvo_oracle_hardware_threads())
+
+
+def _direct_stats(st):
+    singular = st[:, 2].astype(np.int64)
+    return {"exit": st[:, 0].astype(np.int32), "iter": st[:, 1].astype(np.int32), "det_zero": (singular & 1) != 0,
+            "hinv_nonfinite": (singular & 2) != 0, "h_inv_nonfinite": (singular & 4) != 0, "conv_margin": st[:, 3].copy(),
+            "backoff_margin": st[:, 4].copy(), "tie": st[:, 5] != 0, "dist": st[:, 6:10].copy(), "bound": st[:, 10].astype(np.int32),
+            "offset": st[:, 11].astype(np.int32), "reject": st[:, 12] != 0, "nan_warp": st[:, 13] != 0, "clamped": st[:, 14] != 0,
+            "zeroed": st[:, 15].astype(np.int32), "nan_dir": st[:, 16] != 0, "edgelet": st[:, 17] != 0,
+            "on_bound": st[:, 18].astype(np.int32)}
+
+
+def _stats_fn(lib, name, batch_t, result_t):
+    fn = getattr(lib, name)
+    fn.restype = C.c_int
+    fn.argtypes = [C.POINTER(batch_t), C.POINTER(result_t), C.POINTER(C.c_double), C.c_int]
+    return fn
+
+
+def feature_align_stats(abi, kind, cur_pyr, image_index, level, border, ref, px, n_iter, width, height, dirs=None, n_threads=0,
+                        stats=True):
+    """align2D (kind "2d") or align1D (kind "1d", along dirs) over a batch, through plsvo_oracle_align{2,1}d_batch or, with
+    stats, through plsvo_oracle_align{2,1}d_stats, which run the same code and also record each feature's decisions.
+    cur_pyr: {level: u8 [n_images,h,w]} (views with unit column stride are fine).  Returns ((converged, px) for "2d" or
+    (converged, px, h_inv) for "1d", stats); stats is None without stats, else a dict of arrays over the features:
+      exit, iter            DS_EXIT_* and the iteration the loop ended at (n_iter - 1 at the cap, -1 without an iteration)
+      det_zero, hinv_nonfinite, h_inv_nonfinite   a singular H: det == 0, a non-finite Hinv entry, a non-finite h_inv
+      conv_margin, backoff_margin   smallest relative margin of the convergence and of the back-off test (inf: none)
+      tie                   a back-off test compared equal chi2 values
+      dist [n,4]            smallest distance of floor(u), floor(v) to each in-frame bound (DS_BOUNDS; negative = outside)
+      bound                 the bounds a frame exit failed, bit k = DS_BOUNDS[k]
+      offset                (floor(u) - 4) & 3 at the first iteration inside the frame, else -1"""
+    assert kind in ("2d", "1d")
+    lib = load(abi)
+    pyr = cur_pyr if isinstance(cur_pyr, dict) else dict(enumerate(cur_pyr))
+    image_index = np.ascontiguousarray(image_index, np.int32)
+    level = np.ascontiguousarray(level, np.int32)
+    border = np.ascontiguousarray(border, np.uint8)
+    ref = np.ascontiguousarray(ref, np.uint8)
+    px = np.ascontiguousarray(px, np.float64)
+    n = len(image_index)
+    b, keep = abi.make_align2d_batch(pyr, image_index, level, border, ref, px, n_iter, width, height)
+    out_px, conv = np.zeros((n, 2)), np.zeros(n, np.uint8)
+    dp, u8p = C.POINTER(C.c_double), C.POINTER(C.c_uint8)
+    st = np.zeros((n, lib.plsvo_oracle_direct_stats_stride())) if stats else None
+    if kind == "2d":
+        r = abi.Align2DResult(out_px.ctypes.data_as(dp), conv.ctypes.data_as(u8p))
+        name, bt, rt, arg = "plsvo_oracle_align2d", abi.Align2DBatch, abi.Align2DResult, b
+    else:
+        d = np.ascontiguousarray(dirs, np.float32)
+        h_inv = np.zeros(n)
+        arg = abi.Align1DBatch(b, d.ctypes.data_as(C.POINTER(C.c_float)))
+        r = abi.Align1DResult(out_px.ctypes.data_as(dp), conv.ctypes.data_as(u8p), h_inv.ctypes.data_as(dp))
+        name, bt, rt = "plsvo_oracle_align1d", abi.Align1DBatch, abi.Align1DResult
+    nt = _n_threads(abi, n_threads)
+    if stats:
+        rc = _stats_fn(lib, name + "_stats", bt, rt)(C.byref(arg), C.byref(r), st.ctypes.data_as(dp), nt)
+    else:
+        fn = getattr(lib, name + "_batch")
+        fn.restype, fn.argtypes = C.c_int, [C.POINTER(bt), C.POINTER(rt), C.c_int]
+        rc = fn(C.byref(arg), C.byref(r), nt)
+    if rc != 0:
+        raise RuntimeError(f"oracle {name} failed rc={rc}")
+    outs = (conv.astype(bool), out_px) if kind == "2d" else (conv.astype(bool), out_px, h_inv)
+    return outs, (_direct_stats(st) if stats else None)
+
+
+def align2d_batch(abi, cur_pyr, image_index, level, border, ref, px, n_iter, width, height, n_threads=0):
+    """align2d on all cores (plsvo_oracle_align2d_batch) -> (converged [n] bool, px [n,2])."""
+    return feature_align_stats(abi, "2d", cur_pyr, image_index, level, border, ref, px, n_iter, width, height, None, n_threads, False)[0]
+
+
+def align1d_batch(abi, cur_pyr, image_index, level, dirs, border, ref, px, n_iter, width, height, n_threads=0):
+    """align1d on all cores (plsvo_oracle_align1d_batch) -> (converged [n] bool, px [n,2], h_inv [n])."""
+    return feature_align_stats(abi, "1d", cur_pyr, image_index, level, border, ref, px, n_iter, width, height, dirs, n_threads, False)[0]
+
+
+def match_direct_stats(abi, data, n_threads=0, out=None):
+    """match_direct through plsvo_oracle_match_direct_stats -> (abi.MatchOut, stats): the stats of feature_align_stats
+    (exit kind "none" where the candidate never reaches alignment) and, per candidate:
+      reject     failed the reference in-frame test       nan_warp   the affine warp is NaN (the patch stays zero)
+      clamped    the search level stopped at n_pyr_levels - 1 with D > 3
+      zeroed     border-patch pixels set to 0 because they lie outside the reference image
+      nan_dir    an edgelet whose warped gradient direction is NaN;   edgelet   aligned with align1D
+      on_bound   border-patch samples exactly on the last column or row of the reference image (zeroed, as outside)
+    out: an abi.MatchOut to write into (e.g. with A_cur_ref prefilled), else a fresh one."""
+    lib = load(abi)
+    b, keep = abi.make_match_batch(data)
+    out = out or abi.MatchOut(data.n)
+    st = np.zeros((data.n, lib.plsvo_oracle_direct_stats_stride()))
+    fn = _stats_fn(lib, "plsvo_oracle_match_direct_stats", abi.MatchBatch, abi.MatchResult)
+    rc = fn(C.byref(b), C.byref(out.struct), st.ctypes.data_as(C.POINTER(C.c_double)), _n_threads(abi, n_threads))
+    if rc != 0:
+        raise RuntimeError(f"oracle match_direct_stats failed rc={rc}")
+    return out, _direct_stats(st)
+
+
 # ---- oracle/_ref: the reference's own translation units (oracle/ref_harness.cpp, Makefile target `ref`) ----
 REF_LIB_PATH = os.path.join(_HERE, "_ref", "libplsvo_ref.so")
 REFERENCE_ROOT = os.environ.get("PLSVO_REFERENCE_ROOT", "/root/reference")
@@ -526,13 +631,13 @@ def ref_align1d(abi, cur_pyr, image_index, level, dirs, border, ref, px, n_iter)
     return _align1d_loop(load_ref(abi).plsvo_ref_align1d, cur_pyr, image_index, level, dirs, border, ref, px, n_iter)
 
 
-def match_direct(abi, data, n_threads: int = 1):
-    """Matcher::findMatchDirect restated, over a synth.MatchData batch -> abi.MatchOut."""
+def match_direct(abi, data, n_threads: int = 1, out=None):
+    """Matcher::findMatchDirect restated, over a synth.MatchData batch -> abi.MatchOut (out, if given, is written into)."""
     lib = load(abi)
     lib.plsvo_oracle_match_direct_batch.restype = C.c_int
     lib.plsvo_oracle_match_direct_batch.argtypes = [C.POINTER(abi.MatchBatch), C.POINTER(abi.MatchResult), C.c_int]
     b, keep = abi.make_match_batch(data)
-    out = abi.MatchOut(data.n)
+    out = out or abi.MatchOut(data.n)
     rc = lib.plsvo_oracle_match_direct_batch(C.byref(b), C.byref(out.struct), n_threads)
     if rc != 0:
         raise RuntimeError(f"oracle match_direct failed rc={rc}")

@@ -1222,11 +1222,76 @@ void plsvo_oracle_half_sample(const uint8_t* in, int cols, int rows, size_t in_p
   }
 }
 
+// One feature's record of plsvo_oracle_align2d_stats / _align1d_stats / _match_direct_stats (doubles; written, never
+// read — test infrastructure: which exits, bounds and degenerate systems a test batch reaches):
+//   [kDsExit]      how the Gauss-Newton loop ended: kExitNone (no iteration ran), kExitFrame (the patch left the frame),
+//                  kExitConverged, kExitCap (n_iter iterations ran), kExitBackoff (align1D's new_chi2 > chi2)
+//   [kDsIter]      the iteration it ended at (n_iter - 1 at the cap; -1 without an iteration)
+//   [kDsSingular]  bit 0: det == 0; bit 1: an entry of Hinv is not finite; bit 2: align1D's h_inv is not finite
+//   [kDsConvMargin], [kDsBackMargin]  smallest |a - b| / |b| of the convergence test (update^2 < min_update_squared) and
+//                  of the back-off test (new_chi2 > chi2); inf without such a test
+//   [kDsTie]       1 if a back-off test compared equal chi2 values
+//   [kDsDist + k]  smallest distance of floor(u), floor(v) to the in-frame bounds over all iterations, k = left (u - 4),
+//                  top (v - 4), right (cols - 5 - u), bottom (rows - 5 - v); negative = outside; inf without an iteration
+//   [kDsBound]     the bounds the frame exit failed: 1 left, 2 top, 4 right, 8 bottom
+//   [kDsOffset]    (floor(u) - 4) & 3 at the first iteration inside the frame (the byte offset of the window), else -1
+// findMatchDirect only:
+//   [kDsReject]    the candidate failed the reference in-frame test (isInFrame(px / 2^level, 6, level))
+//   [kDsNanWarp]   the affine warp is NaN (warpAffine leaves the zeroed patch as it is)
+//   [kDsClamped]   getBestSearchLevel stopped at n_pyr_levels - 1 with D > 3 still true
+//   [kDsZeroed]    number of border-patch pixels set to 0 because they fall outside the reference image
+//   [kDsNanDir]    an edgelet whose warped gradient direction is NaN;  [kDsEdgelet] aligned with align1D
+//   [kDsOnBound]   number of border-patch samples exactly on the last column or row (q0 == cols - 1 or q1 == rows - 1),
+//                  which `q >= cols - 1` zeroes and `q > cols - 1` would interpolate; the four corners, which no template
+//                  gradient reads, are not counted
+enum { kDsExit, kDsIter, kDsSingular, kDsConvMargin, kDsBackMargin, kDsTie, kDsDist, kDsBound = kDsDist + 4, kDsOffset, kDsReject,
+       kDsNanWarp, kDsClamped, kDsZeroed, kDsNanDir, kDsEdgelet, kDsOnBound, kDsStride };
+enum { kExitNone, kExitFrame, kExitConverged, kExitCap, kExitBackoff };
+struct DirectStats {
+  double* s;
+  void begin() {
+    if (!s) return;
+    for (int k = 0; k < kDsStride; ++k) s[k] = 0;
+    s[kDsIter] = -1, s[kDsOffset] = -1;
+    s[kDsConvMargin] = s[kDsBackMargin] = INFINITY;
+    for (int k = 0; k < 4; ++k) s[kDsDist + k] = INFINITY;
+  }
+  static double margin(double a, double b) { return std::fabs(a - b) / std::fabs(b); }
+  void bounds(int iter, int ui, int vi, int cols, int rows) {
+    if (!s) return;
+    const double d[4] = {(double)ui - 4, (double)vi - 4, (double)cols - 5 - ui, (double)rows - 5 - vi};
+    int mask = 0;
+    for (int k = 0; k < 4; ++k) s[kDsDist + k] = std::min(s[kDsDist + k], d[k]), mask |= d[k] < 0 ? 1 << k : 0;
+    if (mask) s[kDsBound] = mask, exit(kExitFrame, iter);
+    else if (s[kDsOffset] < 0) s[kDsOffset] = (double)((ui - 4) & 3);
+  }
+  void converge_test(float q, float thr) {
+    if (s) s[kDsConvMargin] = std::min(s[kDsConvMargin], margin(q, thr));
+  }
+  void backoff_test(float new_chi2, float chi2) {
+    if (!s) return;
+    s[kDsBackMargin] = std::min(s[kDsBackMargin], margin(new_chi2, chi2));
+    if (new_chi2 == chi2) s[kDsTie] = 1;
+  }
+  void singular(double det, const float* hinv, int n) {
+    if (!s) return;
+    int f = det == 0 ? 1 : 0;
+    for (int k = 0; k < n; ++k) f |= std::isfinite(hinv[k]) ? 0 : 2;
+    s[kDsSingular] = f;
+  }
+  void exit(int kind, int iter) {
+    if (s) s[kDsExit] = kind, s[kDsIter] = iter;
+  }
+  void end(int n_iter) {  // the loop ran out of iterations
+    if (s && n_iter > 0 && s[kDsExit] == kExitNone) exit(kExitCap, n_iter - 1);
+  }
+};
+
 // feature_alignment::align2D, scalar path — src/feature_alignment.cpp:160-290.  cur_img: cols x rows, row step
 // cur_step; ref_patch_with_border 10x10, ref_patch 8x8; px = cur_px_estimate in/out.  Returns `converged`.
 // Hinv = H.inverse() follows Eigen's fixed-size 3x3 inverse (cofactors of column 0, determinant, 1/det).
-int plsvo_oracle_align2d(const uint8_t* cur_img, int cols, int rows, size_t cur_step_, const uint8_t* ref_patch_with_border,
-                         const uint8_t* ref_patch, int n_iter, double* px) {
+static int align2d_one(const uint8_t* cur_img, int cols, int rows, size_t cur_step_, const uint8_t* ref_patch_with_border,
+                       const uint8_t* ref_patch, int n_iter, double* px, DirectStats st) {
   const int patch_size_ = 8;
   Image im{cur_img, cols, rows, (int)cur_step_};
   bool converged = false;
@@ -1260,6 +1325,7 @@ int plsvo_oracle_align2d(const uint8_t* cur_img, int cols, int rows, size_t cur_
     Hinv[0][0] = c0 * invdet, Hinv[0][1] = c1 * invdet, Hinv[0][2] = c2 * invdet;
     Hinv[1][0] = cof(0, 1) * invdet, Hinv[1][1] = cof(1, 1) * invdet, Hinv[1][2] = cof(2, 1) * invdet;
     Hinv[2][0] = cof(0, 2) * invdet, Hinv[2][1] = cof(1, 2) * invdet, Hinv[2][2] = cof(2, 2) * invdet;
+    st.singular(det, &Hinv[0][0], 9);
   }
   float mean_diff = 0;
   float u = (float)px[0];
@@ -1270,6 +1336,7 @@ int plsvo_oracle_align2d(const uint8_t* cur_img, int cols, int rows, size_t cur_
   for (int iter = 0; iter < n_iter; ++iter) {
     Patch patch(im);
     patch.setPosition((double)u, (double)v);
+    st.bounds(iter, patch.u_ref_i, patch.v_ref_i, cols, rows);
     if (!patch.isInFrame(4)) break;
     patch.computeInterpWeights();
     const uint8_t* roi = im.data + (size_t)(patch.v_ref_i - 4) * im.stride + (patch.u_ref_i - 4);
@@ -1291,20 +1358,28 @@ int plsvo_oracle_align2d(const uint8_t* cur_img, int cols, int rows, size_t cur_
     u += update[0];
     v += update[1];
     mean_diff += update[2];
-    if (update[0] * update[0] + update[1] * update[1] < min_update_squared) {
+    const float update_squared = update[0] * update[0] + update[1] * update[1];
+    st.converge_test(update_squared, min_update_squared);
+    if (update_squared < min_update_squared) {
       converged = true;
+      st.exit(kExitConverged, iter);
       break;
     }
   }
+  st.end(n_iter);
   px[0] = u, px[1] = v;
   return converged ? 1 : 0;
+}
+int plsvo_oracle_align2d(const uint8_t* cur_img, int cols, int rows, size_t cur_step_, const uint8_t* ref_patch_with_border,
+                         const uint8_t* ref_patch, int n_iter, double* px) {
+  return align2d_one(cur_img, cols, rows, cur_step_, ref_patch_with_border, ref_patch, n_iter, px, DirectStats{nullptr});
 }
 
 // feature_alignment::align1D — src/feature_alignment.cpp:40-157.  dir = direction the patch may move in;
 // returns `converged`, writes px (in/out) and h_inv.  Matrix2f::inverse() follows Eigen's 2x2 path
 // (determinant, 1/det, adjugate * invdet).
-int plsvo_oracle_align1d(const uint8_t* cur_img, int cols, int rows, size_t cur_step_, const float* dir,
-                         const uint8_t* ref_patch_with_border, const uint8_t* ref_patch, int n_iter, double* px, double* h_inv) {
+static int align1d_one(const uint8_t* cur_img, int cols, int rows, size_t cur_step_, const float* dir, const uint8_t* ref_patch_with_border,
+                       const uint8_t* ref_patch, int n_iter, double* px, double* h_inv, DirectStats st) {
   const int halfpatch_size_ = 4, patch_size = 8;
   bool converged = false;
   float ref_patch_dv[64];
@@ -1331,6 +1406,8 @@ int plsvo_oracle_align1d(const uint8_t* cur_img, int cols, int rows, size_t cur_
     Hinv[1][0] = -H[1][0] * invdet;
     Hinv[0][1] = -H[0][1] * invdet;
     Hinv[1][1] = H[0][0] * invdet;
+    st.singular(det, &Hinv[0][0], 4);
+    if (st.s && !std::isfinite(*h_inv)) st.s[kDsSingular] += 4;
   }
   float mean_diff = 0;
   float u = (float)px[0];
@@ -1345,6 +1422,7 @@ int plsvo_oracle_align1d(const uint8_t* cur_img, int cols, int rows, size_t cur_
     const double fu = std::floor((double)u), fv = std::floor((double)v);
     const int u_r = (fu >= -2147483648.0 && fu < 2147483648.0) ? (int)fu : INT32_MIN;
     const int v_r = (fv >= -2147483648.0 && fv < 2147483648.0) ? (int)fv : INT32_MIN;
+    st.bounds(iter, u_r, v_r, cols, rows);
     if (u_r < halfpatch_size_ || v_r < halfpatch_size_ || u_r >= cols - halfpatch_size_ || v_r >= rows - halfpatch_size_) break;
     const float subpix_x = u - u_r;
     const float subpix_y = v - v_r;
@@ -1366,9 +1444,11 @@ int plsvo_oracle_align1d(const uint8_t* cur_img, int cols, int rows, size_t cur_
         new_chi2 += res * res;
       }
     }
+    if (iter > 0) st.backoff_test(new_chi2, chi2);
     if (iter > 0 && new_chi2 > chi2) {
       u -= update[0];
       v -= update[1];
+      st.exit(kExitBackoff, iter);
       break;
     }
     chi2 = new_chi2;
@@ -1378,13 +1458,21 @@ int plsvo_oracle_align1d(const uint8_t* cur_img, int cols, int rows, size_t cur_
     u += update[0] * dir[0];
     v += update[0] * dir[1];
     mean_diff += update[1];
-    if (update[0] * update[0] + update[1] * update[1] < min_update_squared) {
+    const float update_squared = update[0] * update[0] + update[1] * update[1];
+    st.converge_test(update_squared, min_update_squared);
+    if (update_squared < min_update_squared) {
       converged = true;
+      st.exit(kExitConverged, iter);
       break;
     }
   }
+  st.end(n_iter);
   px[0] = u, px[1] = v;
   return converged ? 1 : 0;
+}
+int plsvo_oracle_align1d(const uint8_t* cur_img, int cols, int rows, size_t cur_step_, const float* dir,
+                         const uint8_t* ref_patch_with_border, const uint8_t* ref_patch, int n_iter, double* px, double* h_inv) {
+  return align1d_one(cur_img, cols, rows, cur_step_, dir, ref_patch_with_border, ref_patch, n_iter, px, h_inv, DirectStats{nullptr});
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -1435,24 +1523,27 @@ static void warp_matrix_affine(const plsvo_camera& cam, const double* px_ref, Ve
   A[1][1] = (px_dv[1] - px_cur[1]) / halfpatch_size;
 }
 // warp::getBestSearchLevel — :73-87
-static int best_search_level(const double A[2][2], int max_level) {
+static int best_search_level(const double A[2][2], int max_level, bool* clamped = nullptr) {
   int search_level = 0;
   double D = A[0][0] * A[1][1] - A[1][0] * A[0][1];
   while (D > 3.0 && search_level < max_level) {
     search_level += 1;
     D *= 0.25;
   }
+  if (clamped) *clamped = D > 3.0;
   return search_level;
 }
 // warp::warpAffine with halfpatch_size = 5 (:89-133) + createPatchFromPatchWithBorder (:148-157).
 // patch_with_border must be zero-initialised by the caller (a NaN warp leaves it untouched).
 static void warp_affine_patches(const double A[2][2], const uint8_t* img, int stride, int cols, int rows, const double* px_ref,
-                                int level_ref, int search_level, uint8_t patch_with_border[100], uint8_t patch[64]) {
+                                int level_ref, int search_level, uint8_t patch_with_border[100], uint8_t patch[64],
+                                DirectStats st = DirectStats{nullptr}) {
   const int halfpatch_size = 5, patch_size = 10;
   const double det = A[0][0] * A[1][1] - A[1][0] * A[0][1];
   const double invdet = 1.0 / det;
   const float R00 = (float)(A[1][1] * invdet), R10 = (float)(-A[1][0] * invdet);
   const float R01 = (float)(-A[0][1] * invdet), R11 = (float)(A[0][0] * invdet);
+  if (st.s && std::isnan(R00)) st.s[kDsNanWarp] = 1;
   if (!std::isnan(R00)) {
     const float pr0 = (float)px_ref[0] / (1 << level_ref), pr1 = (float)px_ref[1] / (1 << level_ref);
     uint8_t* patch_ptr = patch_with_border;
@@ -1462,9 +1553,12 @@ static void warp_affine_patches(const double A[2][2], const uint8_t* img, int st
         p0 *= (1 << search_level), p1 *= (1 << search_level);
         const float q0 = (R00 * p0 + R01 * p1) + pr0;
         const float q1 = (R10 * p0 + R11 * p1) + pr1;
-        if (q0 < 0 || q1 < 0 || q0 >= cols - 1 || q1 >= rows - 1)
+        const bool corner = (x == 0 || x == 9) && (y == 0 || y == 9);  // no template gradient reads the corners
+        if (st.s && !corner && (q0 == cols - 1 || q1 == rows - 1)) st.s[kDsOnBound] += 1;
+        if (q0 < 0 || q1 < 0 || q0 >= cols - 1 || q1 >= rows - 1) {
           *patch_ptr = 0;
-        else
+          if (st.s) st.s[kDsZeroed] += 1;
+        } else
           *patch_ptr = (uint8_t)interpolate_mat_8u(img, stride, q0, q1);
       }
   }
@@ -1472,19 +1566,24 @@ static void warp_affine_patches(const double A[2][2], const uint8_t* img, int st
     for (int x = 0; x < 8; ++x) patch[(y - 1) * 8 + x] = patch_with_border[y * 10 + 1 + x];
 }
 
-static void match_direct_one(const plsvo_match_batch* in, const plsvo_match_result* out, int i) {
+static void match_direct_one(const plsvo_match_batch* in, const plsvo_match_result* out, int i, double* stats = nullptr) {
   const plsvo_camera& cam = in->cam;
   const int halfpatch_size_ = 4;
   const size_t I = (size_t)i;
   const double* px_ref = in->ref_px + 2 * I;
   const int level_ref = in->ref_level[i];
+  DirectStats st{stats ? stats + (size_t)kDsStride * I : nullptr};
+  st.begin();
   out->px_cur[2 * I] = in->px_cur[2 * I], out->px_cur[2 * I + 1] = in->px_cur[2 * I + 1];
   out->success[i] = 0;
   if (out->search_level) out->search_level[i] = -1;
   // :169-171  isInFrame(px.cast<int>()/(1<<level), halfpatch_size_+2, level)
   {
     const int ox = (int)px_ref[0] / (1 << level_ref), oy = (int)px_ref[1] / (1 << level_ref);
-    if (!cam_is_in_frame(cam, ox, oy, halfpatch_size_ + 2, level_ref)) return;
+    if (!cam_is_in_frame(cam, ox, oy, halfpatch_size_ + 2, level_ref)) {
+      if (st.s) st.s[kDsReject] = 1;
+      return;
+    }
   }
   const SE3 T_ref_w = se3_from_pose7(in->T_ref_w + 7 * (size_t)in->ref_index[i]);
   const SE3 T_cur_w = se3_from_pose7(in->T_cur_w + 7 * (size_t)in->cur_index[i]);
@@ -1495,13 +1594,15 @@ static void match_direct_one(const plsvo_match_batch* in, const plsvo_match_resu
   const double depth_ref = norm(T_w_ref.t - pos);  // (ref_ftr_->frame->pos() - pt.pos_).norm()
   double A[2][2];
   warp_matrix_affine(cam, px_ref, f_ref, depth_ref, T_cur_ref, level_ref, A);
-  const int search_level = best_search_level(A, in->n_pyr_levels - 1);
+  bool clamped;
+  const int search_level = best_search_level(A, in->n_pyr_levels - 1, &clamped);
+  if (st.s) st.s[kDsClamped] = clamped;
   if (out->search_level) out->search_level[i] = search_level;
   if (out->A_cur_ref) out->A_cur_ref[4 * I] = A[0][0], out->A_cur_ref[4 * I + 1] = A[0][1], out->A_cur_ref[4 * I + 2] = A[1][0], out->A_cur_ref[4 * I + 3] = A[1][1];
   uint8_t patch_with_border[100] = {0};
   uint8_t patch[64];
   warp_affine_patches(A, in->ref_img[level_ref] + (size_t)in->ref_index[i] * in->ref_stride[level_ref], (int)in->ref_pitch[level_ref],
-                      cam.width >> level_ref, cam.height >> level_ref, px_ref, level_ref, search_level, patch_with_border, patch);
+                      cam.width >> level_ref, cam.height >> level_ref, px_ref, level_ref, search_level, patch_with_border, patch, st);
   // ---- align at the search level ----
   const double scale = (double)(1 << search_level);
   double px_scaled[2] = {in->px_cur[2 * I] / scale, in->px_cur[2 * I + 1] / scale};
@@ -1514,10 +1615,11 @@ static void match_direct_one(const plsvo_match_batch* in, const plsvo_match_resu
     const double n = std::sqrt(d0 * d0 + d1 * d1);
     d0 /= n, d1 /= n;
     const float dir[2] = {(float)d0, (float)d1};
+    if (st.s) st.s[kDsEdgelet] = 1, st.s[kDsNanDir] = std::isnan(dir[0]) || std::isnan(dir[1]);
     double h_inv;
-    ok = plsvo_oracle_align1d(cur, ccols, crows, in->cur_pitch[search_level], dir, patch_with_border, patch, in->n_iter, px_scaled, &h_inv);
+    ok = align1d_one(cur, ccols, crows, in->cur_pitch[search_level], dir, patch_with_border, patch, in->n_iter, px_scaled, &h_inv, st);
   } else {
-    ok = plsvo_oracle_align2d(cur, ccols, crows, in->cur_pitch[search_level], patch_with_border, patch, in->n_iter, px_scaled);
+    ok = align2d_one(cur, ccols, crows, in->cur_pitch[search_level], patch_with_border, patch, in->n_iter, px_scaled, st);
   }
   out->px_cur[2 * I] = px_scaled[0] * scale, out->px_cur[2 * I + 1] = px_scaled[1] * scale;
   out->success[i] = (uint8_t)ok;
@@ -1526,6 +1628,15 @@ static void match_direct_one(const plsvo_match_batch* in, const plsvo_match_resu
 int plsvo_oracle_match_direct_batch(const plsvo_match_batch* in, const plsvo_match_result* out, int n_threads) {
   if (!in || !out) return PLSVO_ERR_INVALID;
   parallel_for(in->n_features, n_threads, [&](int i) { match_direct_one(in, out, i); });
+  return PLSVO_OK;
+}
+
+// The stride of the records of the three *_stats entry points below (see DirectStats).
+int plsvo_oracle_direct_stats_stride(void) { return kDsStride; }
+// The same findMatchDirect, also recording every candidate's decisions: stats [n_features][kDsStride].
+int plsvo_oracle_match_direct_stats(const plsvo_match_batch* in, const plsvo_match_result* out, double* stats, int n_threads) {
+  if (!in || !out || !stats) return PLSVO_ERR_INVALID;
+  parallel_for(in->n_features, n_threads, [&](int i) { match_direct_one(in, out, i, stats); });
   return PLSVO_OK;
 }
 
@@ -2077,33 +2188,46 @@ int plsvo_oracle_line_seed_search_stats(const plsvo_line_seed_batch* in, const p
 }
 
 // Batch drivers over the ABI structs (CPU baseline of tools/bench_next.py): one call per feature, threads over features.
+// (The *_stats variants also write each feature's DirectStats record to stats [n_features][kDsStride].)
+static void align_batch_one(const plsvo_align2d_batch* in, const float* dir, double* o_px, uint8_t* o_conv, double* o_hinv, int i,
+                            double* stats) {
+  const int l = in->level[i];
+  const uint8_t* img = in->img[l] + (size_t)in->image_index[i] * in->img_stride[l];
+  double px[2] = {in->px[2 * (size_t)i], in->px[2 * (size_t)i + 1]};
+  DirectStats st{stats ? stats + (size_t)kDsStride * i : nullptr};
+  st.begin();
+  const uint8_t* border = in->ref_patch_with_border + 100 * (size_t)i;
+  const uint8_t* patch = in->ref_patch + 64 * (size_t)i;
+  if (dir) {
+    double h_inv = 0;
+    o_conv[i] = (uint8_t)align1d_one(img, in->width >> l, in->height >> l, in->img_pitch[l], dir + 2 * (size_t)i, border, patch, in->n_iter,
+                                     px, &h_inv, st);
+    if (o_hinv) o_hinv[i] = h_inv;
+  } else {
+    o_conv[i] = (uint8_t)align2d_one(img, in->width >> l, in->height >> l, in->img_pitch[l], border, patch, in->n_iter, px, st);
+  }
+  o_px[2 * (size_t)i] = px[0], o_px[2 * (size_t)i + 1] = px[1];
+}
 int plsvo_oracle_align2d_batch(const plsvo_align2d_batch* in, const plsvo_align2d_result* out, int n_threads) {
   if (!in || !out) return PLSVO_ERR_INVALID;
-  parallel_for(in->n_features, n_threads, [&](int i) {
-    const int l = in->level[i];
-    const uint8_t* img = in->img[l] + (size_t)in->image_index[i] * in->img_stride[l];
-    double px[2] = {in->px[2 * (size_t)i], in->px[2 * (size_t)i + 1]};
-    out->converged[i] = (uint8_t)plsvo_oracle_align2d(img, in->width >> l, in->height >> l, in->img_pitch[l],
-                                                      in->ref_patch_with_border + 100 * (size_t)i, in->ref_patch + 64 * (size_t)i,
-                                                      in->n_iter, px);
-    out->px[2 * (size_t)i] = px[0], out->px[2 * (size_t)i + 1] = px[1];
-  });
+  parallel_for(in->n_features, n_threads, [&](int i) { align_batch_one(in, nullptr, out->px, out->converged, nullptr, i, nullptr); });
   return PLSVO_OK;
 }
 int plsvo_oracle_align1d_batch(const plsvo_align1d_batch* in1, const plsvo_align1d_result* out, int n_threads) {
   if (!in1 || !out) return PLSVO_ERR_INVALID;
-  const plsvo_align2d_batch* in = &in1->features;
-  parallel_for(in->n_features, n_threads, [&](int i) {
-    const int l = in->level[i];
-    const uint8_t* img = in->img[l] + (size_t)in->image_index[i] * in->img_stride[l];
-    double px[2] = {in->px[2 * (size_t)i], in->px[2 * (size_t)i + 1]};
-    double h_inv = 0;
-    out->converged[i] = (uint8_t)plsvo_oracle_align1d(img, in->width >> l, in->height >> l, in->img_pitch[l], in1->dir + 2 * (size_t)i,
-                                                      in->ref_patch_with_border + 100 * (size_t)i, in->ref_patch + 64 * (size_t)i,
-                                                      in->n_iter, px, &h_inv);
-    out->px[2 * (size_t)i] = px[0], out->px[2 * (size_t)i + 1] = px[1];
-    if (out->h_inv) out->h_inv[i] = h_inv;
-  });
+  parallel_for(in1->features.n_features, n_threads,
+               [&](int i) { align_batch_one(&in1->features, in1->dir, out->px, out->converged, out->h_inv, i, nullptr); });
+  return PLSVO_OK;
+}
+int plsvo_oracle_align2d_stats(const plsvo_align2d_batch* in, const plsvo_align2d_result* out, double* stats, int n_threads) {
+  if (!in || !out || !stats) return PLSVO_ERR_INVALID;
+  parallel_for(in->n_features, n_threads, [&](int i) { align_batch_one(in, nullptr, out->px, out->converged, nullptr, i, stats); });
+  return PLSVO_OK;
+}
+int plsvo_oracle_align1d_stats(const plsvo_align1d_batch* in1, const plsvo_align1d_result* out, double* stats, int n_threads) {
+  if (!in1 || !out || !stats) return PLSVO_ERR_INVALID;
+  parallel_for(in1->features.n_features, n_threads,
+               [&](int i) { align_batch_one(&in1->features, in1->dir, out->px, out->converged, out->h_inv, i, stats); });
   return PLSVO_OK;
 }
 int plsvo_oracle_pyramid_batch(const plsvo_pyramid_batch* in, const plsvo_pyramid_result* out, int n_threads) {

@@ -528,12 +528,12 @@ def make_match_batch(d):
     b.n_features, b.n_ref_images, b.n_cur_images = d.n, d.T_ref_w.shape[0], d.T_cur_w.shape[0]
     b.n_pyr_levels, b.n_iter = d.n_pyr_levels, d.n_iter
     b.cam = Camera(d.cam.width, d.cam.height, 0, 0, d.cam.fx, d.cam.fy, d.cam.cx, d.cam.cy)
-    for l, im in d.ref_pyr.items():
-        b.ref_img[l] = _ptr(im, np.uint8)
-        b.ref_pitch[l], b.ref_stride[l] = im.strides[1], im.strides[0]
-    for l, im in d.cur_pyr.items():
-        b.cur_img[l] = _ptr(im, np.uint8)
-        b.cur_pitch[l], b.cur_stride[l] = im.strides[1], im.strides[0]
+    for pyr, img, pitch, stride in ((d.ref_pyr, b.ref_img, b.ref_pitch, b.ref_stride), (d.cur_pyr, b.cur_img, b.cur_pitch, b.cur_stride)):
+        for l, im in pyr.items():  # any u8 [n,h,w] view with unit column stride (padded rows, every other frame, ...)
+            if not isinstance(im, np.ndarray) or im.dtype != np.uint8 or im.ndim != 3 or im.strides[2] != 1 or min(im.strides) < 0:
+                raise TypeError(f"pyramid level {l}: expected a u8 [n,h,w] array with unit column stride")
+            img[l] = im.ctypes.data_as(_u8p)
+            pitch[l], stride[l] = im.strides[1], im.strides[0]
     b.T_ref_w, b.T_cur_w = _ptr(d.T_ref_w, np.float64), _ptr(d.T_cur_w, np.float64)
     b.ref_index, b.cur_index = _ptr(d.ref_index, np.int32), _ptr(d.cur_index, np.int32)
     b.ref_px, b.ref_f, b.ref_level = _ptr(d.ref_px, np.float64), _ptr(d.ref_f, np.float64), _ptr(d.ref_level, np.int32)

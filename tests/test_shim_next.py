@@ -160,3 +160,41 @@ def test_direct_matcher_single_keyframe_single_observation(oracle, abi, synth):
         a, b = getattr(s, f), getattr(r, f)
         np.testing.assert_array_equal(a[~np.isnan(b)], b[~np.isnan(b)], err_msg=f)
     assert set(np.unique(r.pt_ref)) <= {-1, 0}
+
+
+def _nan_warp_scene(synth):
+    """A Reprojector pass where every eighth candidate, right after an ordinary one of the same current frame, is a point the
+    warp of findMatchDirect cannot handle: at the camera centre of its keyframe (a keyframe at the identity: A would be 0)
+    or NaN.  Returns (data, the special rows)."""
+    import torch
+
+    from test_gpu_direct_match_cases import _append_frames
+
+    d = synth.make_match_batch(n=1200, seed=7320)
+    R0, t0 = torch.eye(3, dtype=torch.float64)[None], torch.zeros(1, 3, dtype=torch.float64)
+    ident = _append_frames(synth, d, "ref", synth.pose7_from_Rt(R0, t0).numpy())
+    rows = np.arange(9, d.n, 8)
+    d.cur_index[rows] = d.cur_index[rows - 1]
+    d.ref_index[rows[::2]] = ident
+    d.ref_px[rows] = (d.cam.cx + 3.25, d.cam.cy - 7.5)
+    d.pos[rows[::2]] = 0.0
+    d.pos[rows[1::2]] = (np.nan, 1.0, 2.0)
+    return d, rows
+
+
+@pytest.mark.parametrize("cpu", [True, pytest.param(False, marks=pytest.mark.gpu)], ids=["cpu", "gpu"])
+def test_direct_matcher_never_warps_a_point_at_the_keyframe_centre_or_nan(pkg, oracle, abi, synth, cpu):
+    """A point at its keyframe's camera centre, or a NaN point, would give findMatchDirect a NaN affine warp, where the
+    reference's warpAffine keeps the previous candidate's patch and the kernel aligns a zero patch.  Neither reaches the warp:
+    getCloseViewObs, which DirectMatcher runs on the host as Reprojector does, rejects it first (its viewing direction is
+    zero or NaN, so the cosine is not above 0.5).  Both sides agree on every candidate; the special ones are not found and
+    leave A_cur_ref_ as the candidate before them left it, i.e. no warp was computed for them."""
+    _need_ref(oracle, cpu=cpu)
+    d, rows = _nan_warp_scene(synth)
+    r = oracle.ref_match_scene(abi, d, 1)
+    s = oracle.shimref_match_scene(abi, d, 1, cpu=cpu)
+    _check_match_scene(s, r, 1, d.T_ref_w.shape[0])
+    for out in (r, s):
+        assert not out.pt_found[rows].any()
+        np.testing.assert_array_equal(out.pt_A[rows], out.pt_A[rows - 1])
+        assert np.isfinite(out.pt_A[rows]).all()
