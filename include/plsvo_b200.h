@@ -339,6 +339,40 @@ int plsvo_track_raw_batch_run(plsvo_ctx* ctx, const plsvo_raw_frames* raw, const
                               const plsvo_poseopt_result* po_out, const plsvo_pyramid_result* rect_out);
 
 /* ------------------------------------------------------------------------------------------
+ * Alignment and tracking of frames from an ATAN (FOV) camera: vk::ATANCamera, the model app/run_pipeline.cpp builds when
+ * cam_model selects it.  On that path the frames are not rectified: SparseImgAlign projects every patch through the
+ * distorted model (cam_->world2cam, src/sparse_img_align.cpp:425,584) and the feature constructors form bearings with
+ * its cam2world.  These calls are plsvo_align_batch_run / plsvo_track_batch_run with that camera model.
+ *
+ * plsvo_atan_camera holds the constructor's arguments ATANCamera(width, height, fx, fy, cx, cy, d0), fx..cy normalised
+ * by the image size.  The library derives the rest as the constructor does: fx_ = width fx, fy_ = height fy,
+ * cx_ = cx width - 0.5, cy_ = cy height - 0.5, s_ = d0, tans_ = 2 tan(s_/2) (no distortion when s_ == 0), and
+ *   world2cam(uv): r = |uv|, factor = (r < 0.001 || s_ == 0) ? 1 : atan(r tans_) / (s_ r), px = (cx_ + fx_ factor u, ...)
+ *   cam2world(px): d = ((x - cx_)/fx_, (y - cy_)/fy_), r = s_ ? tan(|d| s_) / tans_ : |d|,
+ *                  (factor d, 1).normalized() with factor = |d| > 0.01 ? r / |d| : 1
+ *   errorMultiplier2() = fx_.
+ * - `batch` (al_batch) is as for plsvo_align_batch_run, including frame chains, NULL bearings (formed on the device with
+ *   the ATAN cam2world) and NULL levels derived on the device.  batch->cam.width / height must equal the camera's; its
+ *   other fields are ignored.
+ * - The pose optimiser is camera-free: po_batch->fx is errorMultiplier2() = fx_ = width fx.
+ * - These calls always run upload -> launch -> download on the context's stream, as the raw-frame calls do: the
+ *   arrival-gated path plsvo_align_batch_run takes for 256 pairs and more is not used.
+ * - A size mismatch, a non-finite parameter, fx <= 0 or fy <= 0 returns PLSVO_ERR_INVALID before anything is queued.
+ *   A library built without the ATAN kernels returns PLSVO_ERR_CUDA.
+ * ---------------------------------------------------------------------------------------- */
+typedef struct plsvo_atan_camera {
+  int32_t width, height;
+  double fx, fy, cx, cy, d0;
+} plsvo_atan_camera;
+
+int plsvo_align_atan_batch_run(plsvo_ctx* ctx, const plsvo_atan_camera* cam, const plsvo_align_batch* batch,
+                               const plsvo_align_params* params, const plsvo_align_result* out);
+int plsvo_track_atan_batch_run(plsvo_ctx* ctx, const plsvo_atan_camera* cam, const plsvo_align_batch* al_batch,
+                               const plsvo_align_params* al_params, const plsvo_poseopt_batch* po_batch,
+                               const plsvo_poseopt_params* po_params, const plsvo_align_result* al_out,
+                               const plsvo_poseopt_result* po_out);
+
+/* ------------------------------------------------------------------------------------------
  * Feature alignment (SURVEY.md §8f "next", rank 1): feature_alignment::align2D,
  * include/plsvo/feature_alignment.h:49-55, src/feature_alignment.cpp:160-290 (scalar path) — the 8x8
  * inverse-compositional refinement Matcher::findMatchDirect runs per feature (src/matcher.cpp:201).

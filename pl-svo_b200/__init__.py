@@ -4,7 +4,7 @@ Package directory is `pl-svo_b200/` (hyphenated, as the repo contract names it);
 the `plsvo_b200` shim module at the repo root.
 """
 from . import abi, dist, synth  # noqa: F401
-from .api import (Context, DepthFilter, Matcher, PinholeCamera, SparseImgAlign, createImgPyramid, default_context, feature_alignment,  # noqa: F401
+from .api import (ATANCamera, Context, DepthFilter, Matcher, PinholeCamera, SparseImgAlign, createImgPyramid, default_context, feature_alignment,  # noqa: F401
                   optimizeStructure, pose_optimizer, track_raw)
 
 __version__ = "0.1.0"

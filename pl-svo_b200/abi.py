@@ -166,6 +166,12 @@ class RawFrames(C.Structure):
     _fields_ = [("cam", PinholeCamera), ("ref_raw", _u8p), ("cur_raw", _u8p), ("pitch", C.c_size_t), ("stride", C.c_size_t)]
 
 
+class AtanCamera(C.Structure):
+    """plsvo_atan_camera: the vk::ATANCamera constructor arguments (fx, fy, cx, cy normalised by the image size)."""
+    _fields_ = [("width", C.c_int32), ("height", C.c_int32), ("fx", C.c_double), ("fy", C.c_double), ("cx", C.c_double),
+                ("cy", C.c_double), ("d0", C.c_double)]
+
+
 def make_raw_frames(cam: PinholeCamera, raw, batch: int):
     """plsvo_raw_frames for `batch` pairs from raw u8 frames: one array [B+1,H,W] (a frame chain) or a pair (ref, cur) of
     [B,H,W] arrays with the same strides.  Rows may be padded.  Returns (struct, chain, keepalive)."""
@@ -466,6 +472,9 @@ ABI_SYMBOLS = [
                                             _P(PyramidResult)]),
     ("plsvo_track_raw_batch_run", C.c_int, [C.c_void_p, _P(RawFrames), _P(AlignBatch), _P(AlignParams), _P(PoseOptBatch),
                                             _P(PoseOptParams), _P(AlignResult), _P(PoseOptResult), _P(PyramidResult)]),
+    ("plsvo_align_atan_batch_run", C.c_int, [C.c_void_p, _P(AtanCamera), _P(AlignBatch), _P(AlignParams), _P(AlignResult)]),
+    ("plsvo_track_atan_batch_run", C.c_int, [C.c_void_p, _P(AtanCamera), _P(AlignBatch), _P(AlignParams), _P(PoseOptBatch),
+                                             _P(PoseOptParams), _P(AlignResult), _P(PoseOptResult)]),
     ("plsvo_align2d_batch_run", C.c_int, [C.c_void_p, _P(Align2DBatch), _P(Align2DResult)]),
     ("plsvo_align1d_batch_run", C.c_int, [C.c_void_p, _P(Align1DBatch), _P(Align1DResult)]),
     ("plsvo_match_direct_batch_run", C.c_int, [C.c_void_p, _P(MatchBatch), _P(MatchResult)]),

@@ -65,6 +65,9 @@ struct AlignArgs {
   double* ws_rec;       // [grid][5][rec_cap*threads] parked in-patch sums of segments longer than a warp
   int rec_cap;          // 32-sample trips of the longest segment, <= 32
   int derive_from;      // >= 0: the CTA forms levels (derive_from, max_level] of its pair by halfSample (gated pipeline)
+  // vk::ATANCamera distortion (read by the ATAN kernels only; fx, fy, cx, cy above then hold fx_, fy_, cx_, cy_):
+  // s_ = d0, s_inv_ = 1/s_, tans_ = 2 tan(s_/2), tans_inv_ = 1/tans_, all zero when s_ == 0
+  double atan_s, atan_s_inv, atan_tans, atan_tans_inv;
 };
 
 // Opaque chi2 patches (16 float terms each) the alignment kernel can hold per Gauss-Newton pass: the patches whose 16
@@ -82,6 +85,12 @@ cudaError_t align_kernel_prepare(int threads, int min_blocks, size_t smem_bytes,
 cudaError_t weight_selftest_launch(uint32_t n, uint32_t seed, unsigned long long* d_mismatch, cudaStream_t s);
 cudaError_t align_kernel_launch(const AlignArgs& a, int grid, int threads, int min_blocks, size_t smem_bytes,
                                 cudaStream_t s);
+// The same kernel variants with the vk::ATANCamera projection (plsvo_align_atan_batch_run).  Weak references for the
+// reason given at undistort_map_launch below: the host-pipeline model of the tests need not provide them, and the ATAN
+// entry points then report them missing.  The library always links align_kernel.cu.
+__attribute__((weak)) cudaError_t align_atan_kernel_prepare(int threads, int min_blocks, size_t smem_bytes, int* ctas_per_sm);
+__attribute__((weak)) cudaError_t align_atan_kernel_launch(const AlignArgs& a, int grid, int threads, int min_blocks,
+                                                           size_t smem_bytes, cudaStream_t s);
 
 // ---------------------------------------------------------------------------------------------
 struct PoseOptArgs {

@@ -63,6 +63,7 @@ struct plsvo_ctx_impl {
   int der_src = -1, der_top = -1;    // derived levels are (der_src, der_top], built from uploaded level der_src
   bool lvl_uploaded[PLSVO_MAX_LEVELS] = {false};
   bool chain = false;              // PLSVO_ALIGN_FRAME_CHAIN: one stack of B+1 frames, cur(b) = frame b+1 = ref(b+1)
+  bool atan = false;               // the uploaded batch is seen through a vk::ATANCamera (the ATAN kernel variants)
   DevBuf d_feat;                     // every per-pair input array of the batch, at 256-byte-aligned offsets
   size_t feat_bytes = 0;
   char* h_po_out = nullptr;          // pinned staging of the pose-optimiser outputs (one D2H per download)
@@ -355,6 +356,7 @@ int align_layout(plsvo_ctx_impl* c, const plsvo_align_batch* h) {
   // frame chain: ref_img[l] is one stack of B+1 frames and the current image of pair b is frame b+1 — the kernel's
   // `cur_img[l] + b*stride` then simply starts one frame further into the same stack
   c->chain = (h->flags & PLSVO_ALIGN_FRAME_CHAIN) != 0;
+  c->atan = false;  // the ATAN entry points set it after the upload
   a.B = h->batch, a.n_pts = h->n_pts, a.n_segs = h->n_segs;
   a.width = h->cam.width, a.height = h->cam.height;
   a.fx = h->cam.fx, a.fy = h->cam.fy, a.cx = h->cam.cx, a.cy = h->cam.cy;
@@ -811,7 +813,8 @@ int align_plan(plsvo_ctx_impl* c, const plsvo_align_params* p, AlignPlan* plan, 
     a.smem_img_bytes = img_bytes;
     a.rec_cap = rec_cap;
     int ctas_per_sm = 0;
-    CK(align_kernel_prepare(threads, min_blocks, smem, &ctas_per_sm));
+    CK(c->atan ? align_atan_kernel_prepare(threads, min_blocks, smem, &ctas_per_sm)
+               : align_kernel_prepare(threads, min_blocks, smem, &ctas_per_sm));
     if (ctas_per_sm < 1) {
       rc_last = fail(c, PLSVO_ERR_INVALID, "kernel does not fit on an SM");
       continue;
@@ -846,7 +849,8 @@ int align_launch_kernel(plsvo_ctx_impl* c, const AlignPlan& plan, cudaStream_t s
   a.gate_chunk = gate_chunk;
   const int grid = std::min(a.B, c->num_sms * plan.ctas_per_sm);
   CK(cudaMemsetAsync(a.work_counter, 0, sizeof(unsigned int), s));
-  CK(align_kernel_launch(a, grid, plan.threads, plan.min_blocks, plan.smem, s));
+  CK(c->atan ? align_atan_kernel_launch(a, grid, plan.threads, plan.min_blocks, plan.smem, s)
+             : align_kernel_launch(a, grid, plan.threads, plan.min_blocks, plan.smem, s));
   c->launches += 1;
   return PLSVO_OK;
 }
@@ -1235,6 +1239,92 @@ int plsvo_poseopt_batch_run(plsvo_ctx* ctx, const plsvo_poseopt_batch* b, const 
   if (rc == PLSVO_OK) rc = plsvo_poseopt_launch(ctx, p);
   if (rc == PLSVO_OK) rc = plsvo_poseopt_download(ctx, o);
   return settled(CTX(ctx), rc);
+}
+
+}  // extern "C"
+
+// ------------------------------------------------------------------------------------------------
+// ATAN (FOV) camera: vk::ATANCamera instead of the undistorted pinhole
+// ------------------------------------------------------------------------------------------------
+namespace {
+
+// Validates the camera against the batch and returns in *derived the batch with cam.fx / fy / cx / cy replaced by the
+// ATANCamera members fx_, fy_, cx_, cy_ (what the kernels read as fx, fy, cx, cy).  Nothing is queued here.
+int atan_batch(plsvo_ctx_impl* c, const plsvo_atan_camera* cam, const plsvo_align_batch* b, plsvo_align_batch* derived) {
+  if (cam->width != b->cam.width || cam->height != b->cam.height)
+    return fail(c, PLSVO_ERR_INVALID, "plsvo_atan_camera size differs from batch->cam");
+  if (!std::isfinite(cam->fx) || !std::isfinite(cam->fy) || !std::isfinite(cam->cx) || !std::isfinite(cam->cy) ||
+      !std::isfinite(cam->d0))
+    return fail(c, PLSVO_ERR_INVALID, "plsvo_atan_camera has a non-finite parameter");
+  if (!(cam->fx > 0.0) || !(cam->fy > 0.0)) return fail(c, PLSVO_ERR_INVALID, "plsvo_atan_camera fx and fy must be positive");
+  *derived = *b;
+  derived->cam.fx = (double)cam->width * cam->fx;
+  derived->cam.fy = (double)cam->height * cam->fy;
+  derived->cam.cx = cam->cx * (double)cam->width - 0.5;
+  derived->cam.cy = cam->cy * (double)cam->height - 0.5;
+  if (!std::isfinite(derived->cam.fx) || !std::isfinite(derived->cam.fy) || !(derived->cam.fx > 0.0) || !(derived->cam.fy > 0.0))
+    return fail(c, PLSVO_ERR_INVALID, "plsvo_atan_camera focal length out of range");
+  if (!align_atan_kernel_prepare || !align_atan_kernel_launch)
+    return fail(c, PLSVO_ERR_CUDA, "this library was built without the ATAN alignment kernels");
+  return PLSVO_OK;
+}
+
+// after the upload of the derived batch: select the ATAN kernels and give them the distortion terms of the constructor
+void atan_select(plsvo_ctx_impl* c, const plsvo_atan_camera* cam) {
+  AlignArgs& a = c->aa;
+  c->atan = true;
+  a.atan_s = cam->d0;
+  a.atan_s_inv = a.atan_tans = a.atan_tans_inv = 0.0;
+  if (cam->d0 != 0.0) {
+    a.atan_tans = 2.0 * tan(cam->d0 / 2.0);
+    a.atan_tans_inv = 1.0 / a.atan_tans;
+    a.atan_s_inv = 1.0 / cam->d0;
+  }
+}
+
+}  // namespace
+
+extern "C" {
+
+static int align_atan_body(plsvo_ctx* ctx, const plsvo_atan_camera* cam, const plsvo_align_batch* b, const plsvo_align_params* p,
+                           const plsvo_align_result* o) {
+  plsvo_ctx_impl* c = CTX(ctx);
+  plsvo_align_batch d;
+  int rc = atan_batch(c, cam, b, &d);
+  if (rc == PLSVO_OK) rc = plsvo_align_upload(ctx, &d);
+  if (rc != PLSVO_OK) return rc;
+  atan_select(c, cam);
+  rc = plsvo_align_launch(ctx, p);
+  if (rc == PLSVO_OK) rc = plsvo_align_download(ctx, o);
+  return rc;
+}
+
+int plsvo_align_atan_batch_run(plsvo_ctx* ctx, const plsvo_atan_camera* cam, const plsvo_align_batch* b,
+                               const plsvo_align_params* p, const plsvo_align_result* o) {
+  if (!ctx || !cam || !b || !p || !o) return PLSVO_ERR_INVALID;
+  return settled(CTX(ctx), align_atan_body(ctx, cam, b, p, o));
+}
+
+static int track_atan_body(plsvo_ctx* ctx, const plsvo_atan_camera* cam, const plsvo_align_batch* ab, const plsvo_align_params* ap,
+                           const plsvo_poseopt_batch* pb, const plsvo_poseopt_params* pp, const plsvo_align_result* ao,
+                           const plsvo_poseopt_result* po) {
+  plsvo_ctx_impl* c = CTX(ctx);
+  plsvo_align_batch d;
+  int rc = atan_batch(c, cam, ab, &d);
+  if (rc == PLSVO_OK) rc = plsvo_track_upload(ctx, &d, pb);
+  if (rc != PLSVO_OK) return rc;
+  atan_select(c, cam);
+  rc = plsvo_track_launch(ctx, ap, pp);
+  if (rc == PLSVO_OK && ao) rc = plsvo_align_download(ctx, ao);
+  if (rc == PLSVO_OK) rc = plsvo_poseopt_download(ctx, po);
+  return rc;
+}
+
+int plsvo_track_atan_batch_run(plsvo_ctx* ctx, const plsvo_atan_camera* cam, const plsvo_align_batch* ab,
+                               const plsvo_align_params* ap, const plsvo_poseopt_batch* pb, const plsvo_poseopt_params* pp,
+                               const plsvo_align_result* ao, const plsvo_poseopt_result* po) {
+  if (!ctx || !cam || !ab || !ap || !pb || !pp || !po) return PLSVO_ERR_INVALID;
+  return settled(CTX(ctx), track_atan_body(ctx, cam, ab, ap, pb, pp, ao, po));
 }
 
 }  // extern "C"

@@ -83,6 +83,17 @@ class PinholeCamera : public AbstractCamera {  // undistorted model, as given to
  private:
   double fx_, fy_, cx_, cy_;
 };
+// vk::ATANCamera (rpg_vikit atan_camera.h), the FOV model of cam_model ATAN: constructor with intrinsics normalised by
+// the image size; the shim reads width/height and the members fx_, fy_, cx_, cy_, s_.
+class ATANCamera : public AbstractCamera {
+ public:
+  ATANCamera(double w, double h, double fx, double fy, double cx, double cy, double d0)
+      : fx_(w * fx), fy_(h * fy), cx_(cx * w - 0.5), cy_(cy * h - 0.5), s_(d0) {
+    width_ = (int)w, height_ = (int)h;
+  }
+  double errorMultiplier2() const override { return fx_; }
+  double fx_, fy_, cx_, cy_, s_;
+};
 }  // namespace vk
 
 namespace plsvo {

@@ -175,14 +175,18 @@ class Scene:
             lam = lam - g / gp
         return torch.stack([Cx + lam * d[..., 0], Cy + lam * d[..., 1], Cz + lam * d[..., 2]], -1)
 
-    def render(self, cam: Camera, pose7: torch.Tensor, chunk: int = 64) -> torch.Tensor:
-        """pose7 [B,7] (T_f_w) -> u8 images [B,H,W]."""
+    def render(self, cam: Camera, pose7: torch.Tensor, chunk: int = 64, atan=None) -> torch.Tensor:
+        """pose7 [B,7] (T_f_w) -> u8 images [B,H,W].  atan: an ATAN (FOV) camera (api.ATANCamera) of cam's size: each
+        pixel's ray is then its cam2world (atan_rays) instead of the pinhole's."""
         dev = pose7.device
         B = pose7.shape[0]
         u = torch.arange(cam.width, dtype=torch.float64, device=dev)
         v = torch.arange(cam.height, dtype=torch.float64, device=dev)
         vv, uu = torch.meshgrid(v, u, indexing="ij")
-        dirs = torch.stack([(uu - cam.cx) / cam.fx, (vv - cam.cy) / cam.fy, torch.ones_like(uu)], -1).reshape(1, -1, 3)
+        if atan is not None:
+            dirs = atan_rays(atan, uu, vv).reshape(1, -1, 3)
+        else:
+            dirs = torch.stack([(uu - cam.cx) / cam.fx, (vv - cam.cy) / cam.fy, torch.ones_like(uu)], -1).reshape(1, -1, 3)
         out = torch.empty(B, cam.height, cam.width, dtype=torch.uint8, device=dev)
         for s in range(0, B, chunk):
             R, t = pose7_to_Rt(pose7[s : s + chunk])
@@ -190,6 +194,16 @@ class Scene:
             I = self.texture(P[..., 0], P[..., 1])
             out[s : s + chunk] = I.round().clamp(0, 255).to(torch.uint8).reshape(-1, cam.height, cam.width)
         return out
+
+
+def atan_rays(atan, u: torch.Tensor, v: torch.Tensor) -> torch.Tensor:
+    """Rays (x, y, 1) of pixels (u, v) of the ATAN (FOV) camera `atan` (api.ATANCamera): its cam2world scaled to z = 1.
+    Scenes rendered and features lifted through these rays are what that camera sees, distortion included."""
+    x, y = (u - atan.cx_) / atan.fx_, (v - atan.cy_) / atan.fy_
+    rd = torch.sqrt(x * x + y * y)
+    r = torch.tan(rd * atan.s_) * atan.tans_inv_ if atan.s_ != 0.0 else rd
+    factor = torch.where(rd > 0.01, r / torch.where(rd > 0.01, rd, torch.ones_like(rd)), torch.ones_like(rd))
+    return torch.stack([factor * x, factor * y, torch.ones_like(x)], -1)
 
 
 def half_sample(img: torch.Tensor) -> torch.Tensor:
@@ -281,9 +295,12 @@ def make_align_batch(
     T_ref_w_gt: np.ndarray | None = None,
     T_cur_w_gt: np.ndarray | None = None,
     chain: bool = False,
+    atan=None,
 ) -> AlignData:
     """SURVEY.md §8d config C2 generator: B independent frame pairs, each with its own reference view,
-    features and motion (seeds derived from `seed`)."""
+    features and motion (seeds derived from `seed`).  atan: an ATAN (FOV) camera (api.ATANCamera) of cam's size — the
+    frames are rendered and the features lifted through it (bearings = its cam2world), so the batch is what that camera
+    sees; `cam` then only gives the image size."""
     dev = torch.device(device)
     scene = scene or Scene()
     n_pyr_levels = n_pyr_levels or (max_level + 1)
@@ -308,12 +325,12 @@ def make_align_batch(
         # one trajectory (the given poses satisfy T_ref_w_gt[b+1] == T_cur_w_gt[b]): every frame is rendered ONCE and the two
         # stacks are views of the one sequence, so "cur of pair b" and "ref of pair b+1" are the same bytes by construction
         # rather than by the renderer happening to be bit-reproducible across batch positions
-        frames = build_pyramid(scene.render(cam, torch.cat([T_ref_w, T_cur_w_gt[-1:]], 0)), n_pyr_levels)
+        frames = build_pyramid(scene.render(cam, torch.cat([T_ref_w, T_cur_w_gt[-1:]], 0), atan=atan), n_pyr_levels)
         ref_pyr = [f[:-1] for f in frames]
         cur_pyr = [f[1:] for f in frames]
     else:
-        ref0 = scene.render(cam, T_ref_w)
-        cur0 = scene.render(cam, T_cur_w_gt)
+        ref0 = scene.render(cam, T_ref_w, atan=atan)
+        cur0 = scene.render(cam, T_cur_w_gt, atan=atan)
         ref_pyr = build_pyramid(ref0, n_pyr_levels)
         cur_pyr = build_pyramid(cur0, n_pyr_levels)
     levels = range(min_level, max_level + 1) if keep_levels_only else range(n_pyr_levels)
@@ -338,6 +355,9 @@ def make_align_batch(
 
     def lift(px_np):
         px = torch.tensor(px_np, **f64)
+        if atan is not None:
+            d = atan_rays(atan, px[..., 0], px[..., 1])
+            return d / d.norm(dim=-1, keepdim=True), scene.intersect(R_ref, t_ref, d)
         d = torch.stack([(px[..., 0] - cam.cx) / cam.fx, (px[..., 1] - cam.cy) / cam.fy, torch.ones_like(px[..., 0])], -1)
         return _bearing(cam, px), scene.intersect(R_ref, t_ref, d)
 
