@@ -658,6 +658,30 @@ int align_size(plsvo_ctx_impl* c, const plsvo_align_batch* h, int size_level) {
   return PLSVO_OK;
 }
 
+// The launch limits of pyramid_kernel, for every caller.  One CTA forms levels 1..6 of a 64x64 level-0 tile, so a launch
+// makes at most 7 levels; a deeper pyramid continues with a second launch whose level 0 is the last level of the first.
+// That level was written by the kernel, so its pitch, stride and base are 16-byte multiples, as the kernel's row loads
+// need.  The frames sit on gridDim.z (at most 65535), so a launch takes at most kPyramidFramesPerLaunch of them.
+constexpr int kPyramidLevelsPerLaunch = 7;
+constexpr int kPyramidFramesPerLaunch = 32768;
+
+int pyramid_launch(plsvo_ctx_impl* c, const PyramidArgs& a, cudaStream_t s) {
+  for (int l0 = 0; l0 + 1 < a.n_levels; l0 += kPyramidLevelsPerLaunch - 1) {
+    PyramidArgs p;
+    memset(&p, 0, sizeof p);
+    p.n_levels = std::min(kPyramidLevelsPerLaunch, a.n_levels - l0);
+    p.width = a.width >> l0, p.height = a.height >> l0;
+    for (int k = 0; k < p.n_levels; ++k) p.pitch[k] = a.pitch[l0 + k], p.stride[k] = a.stride[l0 + k];
+    for (int z0 = 0; z0 < a.B; z0 += kPyramidFramesPerLaunch) {
+      p.B = std::min(kPyramidFramesPerLaunch, a.B - z0);
+      for (int k = 0; k < p.n_levels; ++k) p.level[k] = a.level[l0 + k] + (size_t)z0 * a.stride[l0 + k];
+      CK(pyramid_kernel_launch(p, s));
+      c->launches += 1;
+    }
+  }
+  return PLSVO_OK;
+}
+
 // Pyramid levels that were not uploaded are derived on the device from the highest uploaded level below them by
 // repeated vk::halfSample (pyramid_kernel.cu; bit-identical to frame_utils::createImgPyramid).  The device layout of the
 // derived levels is made once per upload and kept while later launches need no other levels.
@@ -717,14 +741,8 @@ int align_derive_levels(plsvo_ctx_impl* c, int min_level, int max_level, cudaStr
       pa.pitch[l - src] = a.pitch[l];
       pa.stride[l - src] = a.stride[l];
     }
-    // the kernel indexes images with blockIdx.z
-    for (int z0 = 0; z0 < pa.B; z0 += 32768) {
-      PyramidArgs q = pa;
-      q.B = std::min(32768, pa.B - z0);
-      for (int k = 0; k < pa.n_levels; ++k) q.level[k] = pa.level[k] + (size_t)z0 * pa.stride[k];
-      CK(pyramid_kernel_launch(q, s));
-    }
-    c->launches += 1;
+    const int rc = pyramid_launch(c, pa, s);
+    if (rc != PLSVO_OK) return rc;
   }
   return PLSVO_OK;
 }
@@ -1361,9 +1379,9 @@ static int pyramid_batch_run_body(plsvo_ctx* ctx, const plsvo_pyramid_batch* in,
                            in->height, cudaMemcpyHostToDevice, s));
   }
   CK(kernel_timer(c, 0, s));
-  CK(pyramid_kernel_launch(a, s));
+  const int rc = pyramid_launch(c, a, s);
+  if (rc != PLSVO_OK) return rc;
   CK(kernel_timer(c, 1, s));
-  c->launches += 1;
   for (int l = 1; l < in->n_levels; ++l) {
     const int cols = in->width >> l, rows = in->height >> l;
     if (out->pitch[l] < (size_t)cols) return fail(c, PLSVO_ERR_INVALID, "output pitch smaller than the level width");
@@ -1856,10 +1874,8 @@ static int undistort_batch_run_body(plsvo_ctx* ctx, const plsvo_undistort_batch*
     CK(undistort_remap_launch(r, c->num_sms, s));
     c->launches += 1;
   }
-  if (in->n_levels > 1) {
-    CK(pyramid_kernel_launch(a, s));
-    c->launches += 1;
-  }
+  const int rc = pyramid_launch(c, a, s);
+  if (rc != PLSVO_OK) return rc;
   CK(kernel_timer(c, 1, s));
   for (int l = 0; l < in->n_levels; ++l) {
     const int cols = W >> l, rows = H >> l;

@@ -361,6 +361,23 @@ cudaError_t poseopt_kernel_launch(const PoseOptArgs& a0, size_t, cudaStream_t s)
 
 cudaError_t pyramid_kernel_launch(const PyramidArgs& a0, cudaStream_t s) {
   const PyramidArgs a = a0;
+  // what the real kernel cannot run: one 64x64 level-0 tile per CTA holds levels 0..6 (level 7 would be left unwritten),
+  // and the frames sit on gridDim.z (at most 65535)
+  if (a.n_levels < 1 || a.n_levels > 7) {
+    fakecuda::error("pyramid kernel: n_levels " + std::to_string(a.n_levels) + " outside [1,7]");
+    return cudaErrorInvalidValue;
+  }
+  if (a.B < 1 || a.B > 65535) {
+    fakecuda::error("pyramid kernel: B " + std::to_string(a.B) + " outside [1,65535] (gridDim.z)");
+    return cudaErrorInvalidConfiguration;
+  }
+  // level 0 is read with 16-byte loads up to its pitch, levels 1.. are written with 8- and 4-byte stores: every level's
+  // base, pitch and frame stride must be a multiple of 16
+  for (int l = 0; l < a.n_levels; ++l)
+    if (reinterpret_cast<uintptr_t>(a.level[l]) % 16 != 0 || a.pitch[l] % 16 != 0 || a.stride[l] % 16 != 0) {
+      fakecuda::error("pyramid kernel: level " + std::to_string(l) + " base, pitch or stride is not a multiple of 16");
+      return cudaErrorMisalignedAddress;
+    }
   return fakecuda::enqueue(s, [a]() {
     for (int b = 0; b < a.B; ++b)
       for (int l = 1; l < a.n_levels; ++l) {

@@ -83,7 +83,7 @@ def expected(data):
 
 # ---- inputs: random bytes are as good as rendered scenes for a kernel that only digests them ----
 def half(img):
-    a = img.astype(np.int32)
+    a = img[:, : img.shape[1] // 2 * 2, : img.shape[2] // 2 * 2].astype(np.int32)
     return ((a[:, 0::2, 0::2] + a[:, 0::2, 1::2] + a[:, 1::2, 0::2] + a[:, 1::2, 1::2]) >> 2).astype(np.uint8)
 
 
@@ -475,6 +475,43 @@ def s_pyramid_call():
         clean()
         for l in range(5):
             assert np.array_equal(got[l], want[l]), f"pyramid level {l} of a {h}x{w} stack"
+
+
+def s_level_7_derived_from_level_0():
+    """Only level 0 shipped and max_level = 7: levels 1..7 are derived on the device, more than one launch of the pyramid
+    kernel can make (its 64x64 tile holds levels 0..6).  Two stacks, a frame chain and the three-leg API."""
+    cam = synth.Camera(256, 192, 180.0, 180.0, 127.5, 95.5)  # level 7: 2 x 1 pixels
+    d = make_batch(5, 20, 4, 170, cam=cam, min_level=0, max_level=7)  # levels 1..7: the half-samples of level 0
+    d.min_level = 5
+    check(run(shipped(d, [0]), PLSVO_NO_SMALL_UPLOAD=1), d, "two stacks, level 0 -> 7")
+    check(run(shipped(d, [0])), d, "two stacks, small block, level 0 -> 7")
+    check(run(shipped(d, [0]), three_leg=True), d, "three-leg, level 0 -> 7")
+    c = make_batch(5, 20, 4, 171, cam=cam, chain=True, min_level=0, max_level=7)
+    c.min_level = 5
+    check(run(one_stack(c, [0])), c, "chain, level 0 -> 7")
+
+
+def tiny_frames():
+    """70 001 frames of 16 x 8 pixels: more than one launch of the pyramid kernel can index (gridDim.z <= 65535)."""
+    img = np.random.default_rng(172).integers(0, 256, (70001, 8, 16), dtype=np.uint8)
+    return img, [img, half(img), half(half(img))]
+
+
+def s_pyramid_call_past_65535_frames():
+    img, want = tiny_frames()
+    got = pkg.api.createImgPyramid(img, 3, ctx=pkg.api.Context(0))
+    clean()
+    for l in range(3):
+        assert np.array_equal(got[l], want[l]), f"createImgPyramid level {l}"
+
+
+def s_undistort_past_65535_frames():
+    """A camera without distortion: level 0 is the frame itself, levels 1.. its pyramid."""
+    img, want = tiny_frames()
+    got = pkg.PinholeCamera(16, 8, 12.0, 12.0, 7.5, 3.5).undistortImage(img, 3, ctx=pkg.api.Context(0))
+    clean()
+    for l in range(3):
+        assert np.array_equal(got[l], want[l]), f"undistortImage level {l}"
 
 
 def s_track_chained_call():

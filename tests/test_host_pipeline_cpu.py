@@ -12,8 +12,8 @@ exactly the caller's bytes, every buffer must be large enough, every dependency 
 caller's arrays may be pending when a call returns.
 
 The second half seeds faults into a copy of plsvo_abi.cu (a dropped wait for the arrival of the copies, an undersized frame
-stack, a frame that is never shipped, an arrival flag raised too early, a missing drain on an error exit) and requires the
-model to notice each of them.
+stack, a frame that is never shipped, an arrival flag raised too early, a missing drain on an error exit, pyramid levels
+off a 16-byte boundary) and requires the model to notice each of them.
 
 Nothing here is a parity statement about the CUDA kernels — that is what the `-m gpu` tests are for."""
 import importlib.util
@@ -32,6 +32,7 @@ SCENARIOS = ["plain_upload_launch_download", "small_batch_staging_block", "stagi
              "arrival_gated_stream", "padded_host_layouts", "lean_features", "chain_every_host_path", "chain_arrival_gated_stream",
              "chain_padded_host_layouts", "rejected_inputs_leave_nothing_in_flight", "forced_variant_is_the_only_one_tried",
              "seed_schedule_overrides_are_validated", "pose_optimiser_host_paths", "pyramid_call",
+             "level_7_derived_from_level_0", "pyramid_call_past_65535_frames", "undistort_past_65535_frames",
              "track_chained_call", "randomised_configurations", "bench_chain_leg"]
 
 
@@ -127,6 +128,13 @@ FAULTS = {
         "  for (int k = 0; k < n_chunks; ++k) {\n    const size_t b0 = (size_t)k * chunk, b1 = std::min<size_t>(b0 + chunk, B);\n"
         "    CK(cudaMemcpyAsync(d_arrived, &c->h_flags[k], sizeof(unsigned int), cudaMemcpyHostToDevice, c->copy_stream));\n",
         "lazy", ["arrival_gated_stream"]),
+    # pyramid levels placed 8 bytes past a 16-byte boundary: the kernel's 16-byte loads and 8-byte stores would fault
+    "misaligned_pyramid_level": (
+        "    if (l > 0 && !out->level[l]) return fail(c, PLSVO_ERR_INVALID, \"output level missing\");\n"
+        "    a.pitch[l] = (uint32_t)((cols + 15) / 16 * 16);\n    a.stride[l] = (size_t)rows * a.pitch[l];\n    total = (total + 255) / 256 * 256;\n    off[l] = total;\n",
+        "    if (l > 0 && !out->level[l]) return fail(c, PLSVO_ERR_INVALID, \"output level missing\");\n"
+        "    a.pitch[l] = (uint32_t)((cols + 15) / 16 * 16);\n    a.stride[l] = (size_t)rows * a.pitch[l];\n    total = (total + 255) / 256 * 256;\n    off[l] = total + 8;\n",
+        "lazy", ["pyramid_call"]),
     # error exits return while copies from the caller's arrays are still queued
     "error_exit_without_drain": (
         "  if (rc == PLSVO_OK || !c) return rc;\n", "  if (true) return rc;\n",
