@@ -322,8 +322,11 @@ __device__ __forceinline__ void load_row7(const uint8_t* row, int sh, float* g) 
 // Per-pixel values (bilinear intensity, residual, weight, chi2 term) are bit-identical to the reference's
 // float arithmetic and are returned in t[16] (row-major, the reference's summation order); the five in-patch
 // sums are accumulated per pixel in double from the exactly widened float operands, as the reference does
-// for every pixel's J*J^T*w (:487-492).  PLSVO_FP32_SUMS builds the fp32-FMA variant for A/B measurements (0.4 % of
-// pairs then terminate differently from the reference; tools/emulate_kernel_sums.py).
+// for every pixel's J*J^T*w (:487-492).  A point patch returns all five (S = Sxx, Sxy, Syy, Sxr, Syr).  A segment sample
+// is unweighted, so its Sxx, Sxy, Syy depend on the cached gradients alone and are formed once per level
+// (seg_gram_sums); it returns the two that change from pass to pass (S = Sxr, Syr).  PLSVO_FP32_SUMS builds the
+// fp32-FMA variant for A/B measurements (0.4 % of pairs then terminate differently from the reference;
+// tools/emulate_kernel_sums.py).
 template <bool weighted, int NT>
 __device__ __forceinline__ bool eval_patch(const uint8_t* __restrict__ img, int pitch, int cols, int rows,
                                            const float4* __restrict__ cache, int MP, int p, double u, double v,
@@ -370,25 +373,30 @@ __device__ __forceinline__ bool eval_patch(const uint8_t* __restrict__ img, int 
       acc_f = __fsub_rn(acc_f, nterm);
 #ifdef PLSVO_FP32_SUMS
       const float wdx = weighted ? __fmul_rn(-nw, dx) : dx, wdy = weighted ? __fmul_rn(-nw, dy) : dy;
-      Sxx = fmaf(wdx, dx, Sxx);
-      Sxy = fmaf(wdx, dy, Sxy);
-      Syy = fmaf(wdy, dy, Syy);
+      if (weighted) {
+        Sxx = fmaf(wdx, dx, Sxx);
+        Sxy = fmaf(wdx, dy, Sxy);
+        Syy = fmaf(wdy, dy, Syy);
+      }
       Sxr = fmaf(wdx, res, Sxr);
       Syr = fmaf(wdy, res, Syr);
 #else
       const double dxd = (double)dx, dyd = (double)dy, rd = (double)res;
       const double nwdx = weighted ? (double)nw * dxd : -dxd;  // exact products (24+24 bits), negated
       const double nwdy = weighted ? (double)nw * dyd : -dyd;
-      Sxx = fma(-nwdx, dxd, Sxx);
-      Sxy = fma(-nwdx, dyd, Sxy);
-      Syy = fma(-nwdy, dyd, Syy);
+      if (weighted) {
+        Sxx = fma(-nwdx, dxd, Sxx);
+        Sxy = fma(-nwdx, dyd, Sxy);
+        Syy = fma(-nwdy, dyd, Syy);
+      }
       Sxr = fma(-nwdx, rd, Sxr);
       Syr = fma(-nwdy, rd, Syr);
 #endif
     }
     ra_lo = rb_lo, ra_hi = rb_hi;
   }
-  S[0] = (double)Sxx, S[1] = (double)Sxy, S[2] = (double)Syy, S[3] = (double)Sxr, S[4] = (double)Syr;
+  if (weighted) S[0] = (double)Sxx, S[1] = (double)Sxy, S[2] = (double)Syy, S[3] = (double)Sxr, S[4] = (double)Syr;
+  else S[0] = (double)Sxr, S[1] = (double)Syr;
   tsum = acc_f;  // fl-sum of the 16 (positive) terms started from zero: the estimate of this patch's contribution
   return true;
 }
@@ -462,6 +470,39 @@ __device__ __forceinline__ void zero_gradients(float4* cache, int MP, int p) {
   const float4 z = make_float4(0.f, 0.f, 0.f, 0.f);
 #pragma unroll
   for (int y = 0; y < 8; ++y) cache[(4 + y) * MP + p] = z;
+}
+
+// Sxx = sum dx*dx, Sxy = sum dx*dy, Syy = sum dy*dy over the 16 pixels of segment sample p, from its cache rows, with the
+// operations and the order of eval_patch<false> (unweighted: the same values in every pass of the level)
+__device__ __forceinline__ void seg_gram_sums(const float4* __restrict__ cache, int MP, int p, double* g) {
+#ifdef PLSVO_FP32_SUMS
+  float sxx = 0.f, sxy = 0.f, syy = 0.f;
+#else
+  double sxx = 0, sxy = 0, syy = 0;
+#endif
+  const float4* cp = cache + 4 * MP + p;
+#pragma unroll 1
+  for (int y = 0; y < 4; ++y) {
+    const float4 dx4 = cp[0];
+    const float4 dy4 = cp[4 * MP];
+    cp += MP;
+    const float dxv[4] = {dx4.x, dx4.y, dx4.z, dx4.w};
+    const float dyv[4] = {dy4.x, dy4.y, dy4.z, dy4.w};
+#pragma unroll
+    for (int x = 0; x < 4; ++x) {
+#ifdef PLSVO_FP32_SUMS
+      sxx = fmaf(dxv[x], dxv[x], sxx);
+      sxy = fmaf(dxv[x], dyv[x], sxy);
+      syy = fmaf(dyv[x], dyv[x], syy);
+#else
+      const double dxd = (double)dxv[x], dyd = (double)dyv[x];
+      sxx = fma(dxd, dxd, sxx);
+      sxy = fma(dxd, dyd, sxy);
+      syy = fma(dyd, dyd, syy);
+#endif
+    }
+  }
+  g[0] = (double)sxx, g[1] = (double)sxy, g[2] = (double)syy;
 }
 
 // Thread 0, first half of one Gauss-Newton step of vk::NLLSSolver::optimizeGaussNewton: SparseImgAlign::solve()
@@ -603,11 +644,14 @@ __device__ __forceinline__ void align_pairs(const AlignArgs& a) {
   // per-CTA workspaces in global memory
   float4* cache = a.ws_cache + (size_t)blockIdx.x * kCacheRows * MP;
   double* xyz = reinterpret_cast<double*>(smem + L.xyz);
+  // Sxx, Sxy, Syy of segment sample p at [3 * (p - np)], behind the layout when the host plan gave them shared memory
+  double* seg_gram = a.gram_in_smem ? reinterpret_cast<double*>(smem + L.total)
+                                    : a.ws_gram + (size_t)blockIdx.x * 3 * a.max_seg_patches;
   float* tsc = reinterpret_cast<float*>(smem + L.tsc) + tid;  // this thread's term k at tsc[k * NT]
   uint2* flat = reinterpret_cast<uint2*>(smem + L.flat);
   double* seg_px = a.ws_segpx + (size_t)blockIdx.x * 2 * a.max_seg_patches;  // 2-D centre of every segment sample
   const int RS = a.rec_cap * NT;                                     // record slots per component
-  double* rec = a.ws_rec + (size_t)blockIdx.x * 5 * RS;               // five in-patch sums of this pass, per thread slot
+  double* rec = a.ws_rec + (size_t)blockIdx.x * 2 * RS;               // Sxr, Syr of this pass, per thread slot
   uint64_t* bar = reinterpret_cast<uint64_t*>(&ctl->mbar);
   if (tid == 0) {
     mbar_init(bar, 1);
@@ -894,10 +938,12 @@ __device__ __forceinline__ void align_pairs(const AlignArgs& a) {
           // points: skipped at this level (:218-219); their Jacobian columns were zeroed (:85).
           // segment samples are inside by construction; guard only protects against malformed input.
           if (!is_pt || pt_vis[p]) zero_gradients(cache, MP, p);
+          if (!is_pt) seg_gram[3 * (p - np)] = seg_gram[3 * (p - np) + 1] = seg_gram[3 * (p - np) + 2] = 0.0;
           continue;
         }
         if (is_pt) pt_vis[p] = 1;
         precompute_patch(ref_img, pitch, ui, vi, wTL, wTR, wBL, wBR, cache, MP, p);
+        if (!is_pt) seg_gram_sums(cache, MP, p, seg_gram + 3 * (p - np));
         ++my_patch_levels;
       }
       if (stage) {
@@ -1056,7 +1102,7 @@ __device__ __forceinline__ void align_pairs(const AlignArgs& a) {
           float s_tok = 0.f;  // the reference's res_ accumulator (:643-646) handed from sample to sample
           int first_bad = 0x7fffffff;
           unsigned ok_trips = 0u;  // bit t: this lane's sample of trip t was evaluated
-          double S[5] = {0.0, 0.0, 0.0, 0.0, 0.0};
+          double S[2] = {0.0, 0.0};  // Sxr, Syr of this lane's sample
           int p = 0;
           for (int trip = 0; trip < trips; ++trip) {
             const int n = n0 + trip * G;
@@ -1073,8 +1119,7 @@ __device__ __forceinline__ void align_pairs(const AlignArgs& a) {
                 if (trips > 1) {  // segment longer than a warp: park the sums until its weight is known
                   if (trip < a.rec_cap) {
                     double* rp = rec + trip * NT + tid;
-#pragma unroll
-                    for (int k = 0; k < 5; ++k) rp[k * RS] = S[k];
+                    rp[0] = S[0], rp[RS] = S[1];
                   } else {
                     atomicOr(&ctl->chi2_flags, 4);  // host plan violated (never)
                   }
@@ -1123,15 +1168,19 @@ __device__ __forceinline__ void align_pairs(const AlignArgs& a) {
           sJ = __shfl_sync(0xffffffffu, sJ, gbase);
           if (sH != 0.0 || sJ != 0.0) {  // accepted segment: its samples enter the normal equations
             if (trips == 1) {
-              if (ok_trips) rank2_update(acc, xyz[3 * p + 0], xyz[3 * p + 1], xyz[3 * p + 2], S[0] * sH, S[1] * sH, S[2] * sH,
-                                         S[3] * sJ, S[4] * sJ);
+              if (ok_trips) {
+                const double* g = seg_gram + 3 * (p - np);
+                rank2_update(acc, xyz[3 * p + 0], xyz[3 * p + 1], xyz[3 * p + 2], g[0] * sH, g[1] * sH, g[2] * sH,
+                             S[0] * sJ, S[1] * sJ);
+              }
             } else {
               for (int trip = 0; trip < trips && trip < a.rec_cap; ++trip) {
                 if (!((ok_trips >> (trip & 31)) & 1u)) continue;
                 const int pp = np + off + n0 + trip * G;
                 const double* rp = rec + trip * NT + tid;
-                rank2_update(acc, xyz[3 * pp + 0], xyz[3 * pp + 1], xyz[3 * pp + 2], rp[0] * sH, rp[RS] * sH, rp[2 * RS] * sH,
-                             rp[3 * RS] * sJ, rp[4 * RS] * sJ);
+                const double* g = seg_gram + 3 * (pp - np);
+                rank2_update(acc, xyz[3 * pp + 0], xyz[3 * pp + 1], xyz[3 * pp + 2], g[0] * sH, g[1] * sH, g[2] * sH,
+                             rp[0] * sJ, rp[RS] * sJ);
               }
             }
           }

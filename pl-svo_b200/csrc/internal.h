@@ -62,8 +62,10 @@ struct AlignArgs {
   int smem_img_bytes;   // bytes of the image staging buffer
   float4* ws_cache;     // [grid][kCacheRows][max_patches] reference-patch cache (ref, dx, dy rows)
   double* ws_segpx;     // [grid][2][max_seg_patches] 2-D centre of every segment sample (precompute only)
-  double* ws_rec;       // [grid][5][rec_cap*threads] parked in-patch sums of segments longer than a warp
+  double* ws_rec;       // [grid][2][rec_cap*threads] parked Sxr, Syr of the samples of segments longer than a warp
   int rec_cap;          // 32-sample trips of the longest segment, <= 32
+  double* ws_gram;      // [grid][max_seg_patches][3] Sxx, Sxy, Syy of every segment sample, unless gram_in_smem
+  int gram_in_smem;     // 1: they sit in shared memory, 3 * 8 * max_seg_patches bytes behind align_smem_bytes()
   int derive_from;      // >= 0: the CTA forms levels (derive_from, max_level] of its pair by halfSample (gated pipeline)
   // vk::ATANCamera distortion (read by the ATAN kernels only; fx, fy, cx, cy above then hold fx_, fy_, cx_, cy_):
   // s_ = d0, s_inv_ = 1/s_, tans_ = 2 tan(s_/2), tans_inv_ = 1/tans_, all zero when s_ == 0

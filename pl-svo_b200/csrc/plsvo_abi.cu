@@ -73,7 +73,7 @@ struct plsvo_ctx_impl {
   size_t h_in_cap = 0, img_total = 0;
   cudaEvent_t h_in_ev = nullptr;     // the staged copies of the previous small upload
   DevBuf d_ref_img, d_cur_img;
-  DevBuf d_out_T, d_counter, d_ws_cache, d_ws_segpx, d_ws_rec, d_stage;  // d_out_T: every output, one block
+  DevBuf d_out_T, d_counter, d_ws_cache, d_ws_segpx, d_ws_rec, d_ws_gram, d_stage;  // d_out_T: every output, one block
   size_t level_off[PLSVO_MAX_LEVELS];
 
   // ---- pose-opt state ----
@@ -798,7 +798,7 @@ int align_plan(plsvo_ctx_impl* c, const plsvo_align_params* p, AlignPlan* plan, 
   int rc_last = PLSVO_ERR_INVALID;
   for (int i = 0; i < (forced ? 1 : 3); ++i) {
     const int threads = order[i][0], min_blocks = order[i][1];
-    // parked in-patch sums of a segment longer than a warp (one record per thread and 32-sample trip)
+    // parked Sxr, Syr of a segment longer than a warp (one record per thread and 32-sample trip)
     const int rec_cap = std::max(1, (maxN + 31) / 32);
     if (rec_cap > 32) {
       rc_last = fail(c, PLSVO_ERR_INVALID, "a segment has more than 1024 samples");
@@ -828,6 +828,11 @@ int align_plan(plsvo_ctx_impl* c, const plsvo_align_params* p, AlignPlan* plan, 
         continue;
       }
     }
+    // the segment samples' Sxx, Sxy, Syy (formed once per level) go to shared memory when that costs neither a staged
+    // level nor a resident pair, and are read through L2 otherwise
+    const size_t gram_bytes = 3 * sizeof(double) * (size_t)a.max_seg_patches;
+    a.gram_in_smem = (smem + gram_bytes + 1024) * (size_t)min_blocks <= (size_t)limit + 1024 ? 1 : 0;
+    if (a.gram_in_smem) smem += gram_bytes;
     a.smem_img_bytes = img_bytes;
     a.rec_cap = rec_cap;
     int ctas_per_sm = 0;
@@ -843,10 +848,12 @@ int align_plan(plsvo_ctx_impl* c, const plsvo_align_params* p, AlignPlan* plan, 
     const size_t grid_max = (size_t)std::min(a.B, c->num_sms * ctas_per_sm);
     CK(ensure(c->d_ws_cache, grid_max * kCacheRows * a.max_patches * sizeof(float4)));
     CK(ensure(c->d_ws_segpx, grid_max * 2 * a.max_seg_patches * sizeof(double)));
-    CK(ensure(c->d_ws_rec, grid_max * 5 * (size_t)rec_cap * threads * sizeof(double)));
+    CK(ensure(c->d_ws_rec, grid_max * 2 * (size_t)rec_cap * threads * sizeof(double)));
+    CK(ensure(c->d_ws_gram, grid_max * 3 * (size_t)a.max_seg_patches * sizeof(double)));
     a.ws_cache = static_cast<float4*>(c->d_ws_cache.p);
     a.ws_segpx = static_cast<double*>(c->d_ws_segpx.p);
     a.ws_rec = static_cast<double*>(c->d_ws_rec.p);
+    a.ws_gram = static_cast<double*>(c->d_ws_gram.p);
     plan->threads = threads, plan->min_blocks = min_blocks, plan->ctas_per_sm = ctas_per_sm, plan->smem = smem;
     return PLSVO_OK;
   }
