@@ -71,7 +71,8 @@ typedef struct plsvo_align_params {
   double eps;
 } plsvo_align_params;
 
-/* One batch of B frame pairs.  All pairs share the camera and the array strides n_pts/n_segs;
+/* One batch of B frame pairs.  All pairs share the camera (plsvo_align_multicam_batch_run below takes pinhole intrinsics
+ * per pair) and the array strides n_pts/n_segs;
  * per-pair feature counts may be smaller (pt_count/seg_count) and individual features may be
  * flagged invalid (feat3D == NULL in the reference).
  *
@@ -371,6 +372,40 @@ int plsvo_track_atan_batch_run(plsvo_ctx* ctx, const plsvo_atan_camera* cam, con
                                const plsvo_align_params* al_params, const plsvo_poseopt_batch* po_batch,
                                const plsvo_poseopt_params* po_params, const plsvo_align_result* al_out,
                                const plsvo_poseopt_result* po_out);
+
+/* ------------------------------------------------------------------------------------------
+ * Multicam batches: frame pairs from differently calibrated undistorted pinhole cameras in one call, e.g. a fleet of
+ * identical sensors with individual calibrations, or a mix of datasets with the same image size.  These are
+ * plsvo_align_batch_run / plsvo_poseopt_batch_run / plsvo_track_batch_run with the intrinsics taken per pair.
+ * - Alignment: pair b uses cams[b].fx, fy, cx, cy wherever plsvo_align_batch_run uses batch->cam's: world2cam, cam2world
+ *   of bearings not shipped, and the Jacobian factor |fx| / 2^level.  Of batch->cam only width and height are used, and
+ *   every cams[b] must have that width and height.  Everything else of `batch` is as for plsvo_align_batch_run: full or
+ *   lean bearings, depths, ragged counts and masks, PLSVO_ALIGN_FRAME_CHAIN, NULL levels derived on the device, every
+ *   kernel variant (PLSVO_VARIANT).  Pair b's outputs are byte for byte those of plsvo_align_batch_run on the same pair
+ *   with batch->cam = cams[b] and the same kernel variant.
+ * - Pose optimiser: frame b uses fx[b] (its errorMultiplier2) wherever plsvo_poseopt_batch_run uses batch->fx; the
+ *   track call uses |cams[b].fx|, vk::PinholeCamera::errorMultiplier2().  po_batch->fx is ignored by both.
+ * - These calls always run upload -> launch -> download on the context's stream, as the ATAN and raw-frame calls do
+ *   (not the arrival-gated path), and have finished with the caller's arrays when they return, whatever they return.
+ * - NULL cams or fx, a cams[b] whose size differs from batch->cam, a non-finite fx, fy, cx or cy, fx or fy equal to 0,
+ *   a non-finite or non-positive fx[b], or (track) batch sizes that differ return PLSVO_ERR_INVALID before anything is
+ *   queued.  A library built without the multicam kernels returns PLSVO_ERR_CUDA.
+ * - The multicam kernels keep the pair's intrinsics in 128 bytes of shared memory per CTA.  A batch whose shared-memory
+ *   plan lies within that of the limit is planned for the next kernel variant, as any batch that does not fit; with no
+ *   variant left, or PLSVO_VARIANT pinned, it returns PLSVO_ERR_INVALID (DESIGN.md §4.11).
+ * - Out of scope: per-pair image sizes, per-pair ATAN cameras, raw frames (plsvo_*_raw_batch_run), the arrival-gated
+ *   streamed path, separate upload / launch / download legs, dist.align_sharded, the next-row kernels (direct matching,
+ *   seed updates, structure optimisation) and the drop-in shim (one frame per call, nothing to batch).
+ * ---------------------------------------------------------------------------------------- */
+int plsvo_align_multicam_batch_run(plsvo_ctx* ctx, const plsvo_camera* cams /* [B] */, const plsvo_align_batch* batch,
+                                   const plsvo_align_params* params, const plsvo_align_result* out);
+int plsvo_poseopt_multicam_batch_run(plsvo_ctx* ctx, const double* fx /* [B] errorMultiplier2 */,
+                                     const plsvo_poseopt_batch* batch, const plsvo_poseopt_params* params,
+                                     const plsvo_poseopt_result* out);
+int plsvo_track_multicam_batch_run(plsvo_ctx* ctx, const plsvo_camera* cams /* [B] */, const plsvo_align_batch* al_batch,
+                                   const plsvo_align_params* al_params, const plsvo_poseopt_batch* po_batch,
+                                   const plsvo_poseopt_params* po_params, const plsvo_align_result* al_out,
+                                   const plsvo_poseopt_result* po_out);
 
 /* ------------------------------------------------------------------------------------------
  * Feature alignment (SURVEY.md §8f "next", rank 1): feature_alignment::align2D,

@@ -172,6 +172,19 @@ class AtanCamera(C.Structure):
                 ("cy", C.c_double), ("d0", C.c_double)]
 
 
+def make_cameras(cameras, cam, batch: int):
+    """plsvo_camera[B] of a multicam call from `cameras`, an array-like [B, 4] of (fx, fy, cx, cy) rows, each with the
+    image size of `cam` (the batch's camera).  Raises ValueError for another shape."""
+    k = np.asarray(cameras, dtype=np.float64)
+    if k.shape != (batch, 4):
+        raise ValueError(f"cameras must have shape [{batch}, 4] (fx, fy, cx, cy per pair), got {list(k.shape)}")
+    rec = np.zeros(batch, np.dtype([("size", np.int32, 4), ("k", np.float64, 4)]))
+    assert rec.itemsize == C.sizeof(Camera)
+    rec["size"][:, 0], rec["size"][:, 1] = cam.width, cam.height
+    rec["k"] = k
+    return (Camera * batch).from_buffer(rec)  # keeps rec alive
+
+
 def make_raw_frames(cam: PinholeCamera, raw, batch: int):
     """plsvo_raw_frames for `batch` pairs from raw u8 frames: one array [B+1,H,W] (a frame chain) or a pair (ref, cur) of
     [B,H,W] arrays with the same strides.  Rows may be padded.  Returns (struct, chain, keepalive)."""
@@ -475,6 +488,10 @@ ABI_SYMBOLS = [
     ("plsvo_align_atan_batch_run", C.c_int, [C.c_void_p, _P(AtanCamera), _P(AlignBatch), _P(AlignParams), _P(AlignResult)]),
     ("plsvo_track_atan_batch_run", C.c_int, [C.c_void_p, _P(AtanCamera), _P(AlignBatch), _P(AlignParams), _P(PoseOptBatch),
                                              _P(PoseOptParams), _P(AlignResult), _P(PoseOptResult)]),
+    ("plsvo_align_multicam_batch_run", C.c_int, [C.c_void_p, _P(Camera), _P(AlignBatch), _P(AlignParams), _P(AlignResult)]),
+    ("plsvo_poseopt_multicam_batch_run", C.c_int, [C.c_void_p, _f64p, _P(PoseOptBatch), _P(PoseOptParams), _P(PoseOptResult)]),
+    ("plsvo_track_multicam_batch_run", C.c_int, [C.c_void_p, _P(Camera), _P(AlignBatch), _P(AlignParams), _P(PoseOptBatch),
+                                                 _P(PoseOptParams), _P(AlignResult), _P(PoseOptResult)]),
     ("plsvo_align2d_batch_run", C.c_int, [C.c_void_p, _P(Align2DBatch), _P(Align2DResult)]),
     ("plsvo_align1d_batch_run", C.c_int, [C.c_void_p, _P(Align1DBatch), _P(Align1DResult)]),
     ("plsvo_match_direct_batch_run", C.c_int, [C.c_void_p, _P(MatchBatch), _P(MatchResult)]),

@@ -114,13 +114,22 @@ class SparseImgAlign:
         self.last = out
         return out
 
-    def run(self, data, camera: "ATANCamera | None" = None) -> abi.AlignOut:
+    def run(self, data, camera: "ATANCamera | None" = None, cameras=None) -> abi.AlignOut:
         """run(ref_frames, cur_frames) for a whole batch: returns poses, n_tracked (the reference's
         return value, sparse_img_align.cpp:94), H, killed-segment flags.  camera: an ATANCamera when the frames come from
         one (plsvo_align_atan_batch_run; data.cam then only gives the image size); None for the undistorted pinhole
-        data.cam."""
+        data.cam.  cameras: array-like [B, 4] of undistorted pinhole (fx, fy, cx, cy), one row per pair, when the pairs
+        come from differently calibrated cameras of data.cam's image size (plsvo_align_multicam_batch_run)."""
+        _one_camera_model(camera, cameras)
         batch, keep = abi.make_align_batch(data)
         out = abi.AlignOut(data.batch, data.n_segs)
+        if cameras is not None:
+            cams = _cameras_arg(cameras, data)
+            self.ctx.check(self.ctx.lib.plsvo_align_multicam_batch_run(self.ctx.handle, cams, C.byref(batch),
+                                                                       C.byref(self.params), C.byref(out.struct)),
+                           "plsvo_align_multicam_batch_run")
+            self.last = out
+            return out
         if camera is not None:
             camera._check(data)
             self.ctx.check(self.ctx.lib.plsvo_align_atan_batch_run(self.ctx.handle, C.byref(camera.struct), C.byref(batch),
@@ -163,12 +172,19 @@ class pose_optimizer:
 
     @staticmethod
     def optimizeGaussNewton(reproj_thresh: float, n_iter: int, verbose: bool, data, n_iter_ref: int | None = None,
-                            ctx: Context | None = None) -> abi.PoseOptOut:
-        """9-argument overload when n_iter_ref is None, 10-argument overload otherwise."""
+                            ctx: Context | None = None, fx=None) -> abi.PoseOptOut:
+        """9-argument overload when n_iter_ref is None, 10-argument overload otherwise.  fx: array-like [B] of the
+        frames' errorMultiplier2 when they differ (plsvo_poseopt_multicam_batch_run); data.fx is then not used."""
         ctx = ctx or default_context()
         params = abi.poseopt_params(reproj_thresh, n_iter, -1 if n_iter_ref is None else n_iter_ref)
         batch, keep = abi.make_poseopt_batch(data)
         out = abi.PoseOptOut(data.batch, data.n_pts, data.n_segs)
+        if fx is not None:
+            fxa = _frame_fx_arg(fx, data.batch)
+            ctx.check(ctx.lib.plsvo_poseopt_multicam_batch_run(ctx.handle, abi._ptr(fxa, fxa.dtype), C.byref(batch),
+                                                               C.byref(params), C.byref(out.struct)),
+                      "plsvo_poseopt_multicam_batch_run")
+            return out
         ctx.check(
             ctx.lib.plsvo_poseopt_batch_run(ctx.handle, C.byref(batch), C.byref(params), C.byref(out.struct)),
             "plsvo_poseopt_batch_run",
@@ -178,12 +194,15 @@ class pose_optimizer:
 
 def track(align_data, poseopt_data, max_level: int = 4, min_level: int = 2, n_iter: int = 30, reproj_thresh: float = 2.0,
           po_n_iter: int = 10, po_n_iter_ref: int | None = None, chained: bool = True, ctx: Context | None = None,
-          camera: "ATANCamera | None" = None):
+          camera: "ATANCamera | None" = None, cameras=None):
     """FrameHandlerMono::processFrame's two hot-path calls back to back (src/frame_handler_mono.cpp:272-274, :327-329):
     SparseImgAlign::run on every pair, then pose_optimizer::optimizeGaussNewton on every frame, the pose staying on the
     device in between (chained=True: the pose optimiser starts from the aligned pose of the same batch index).
     camera: an ATANCamera when the frames come from one (plsvo_track_atan_batch_run); poseopt_data.fx is then its
-    errorMultiplier2().  Returns (AlignOut, PoseOptOut)."""
+    errorMultiplier2().  cameras: array-like [B, 4] of per-pair undistorted pinhole (fx, fy, cx, cy)
+    (plsvo_track_multicam_batch_run); frame b's errorMultiplier2 is then |cameras[b, 0]| and poseopt_data.fx is not used.
+    Returns (AlignOut, PoseOptOut)."""
+    _one_camera_model(camera, cameras)
     ctx = ctx or default_context()
     ap = abi.align_params(max_level, min_level, n_iter)
     pp = abi.poseopt_params(reproj_thresh, po_n_iter, -1 if po_n_iter_ref is None else po_n_iter_ref)
@@ -193,6 +212,12 @@ def track(align_data, poseopt_data, max_level: int = 4, min_level: int = 2, n_it
         pb.T_f_w = abi._f64p()
     ao = abi.AlignOut(align_data.batch, align_data.n_segs)
     po = abi.PoseOptOut(poseopt_data.batch, poseopt_data.n_pts, poseopt_data.n_segs)
+    if cameras is not None:
+        cams = _cameras_arg(cameras, align_data)
+        ctx.check(ctx.lib.plsvo_track_multicam_batch_run(ctx.handle, cams, C.byref(ab), C.byref(ap), C.byref(pb), C.byref(pp),
+                                                         C.byref(ao.struct), C.byref(po.struct)),
+                  "plsvo_track_multicam_batch_run")
+        return ao, po
     if camera is not None:
         camera._check(align_data)
         ctx.check(ctx.lib.plsvo_track_atan_batch_run(ctx.handle, C.byref(camera.struct), C.byref(ab), C.byref(ap), C.byref(pb),
@@ -202,6 +227,30 @@ def track(align_data, poseopt_data, max_level: int = 4, min_level: int = 2, n_it
     ctx.check(ctx.lib.plsvo_track_batch_run(ctx.handle, C.byref(ab), C.byref(ap), C.byref(pb), C.byref(pp), C.byref(ao.struct),
                                             C.byref(po.struct)), "plsvo_track_batch_run")
     return ao, po
+
+
+def _one_camera_model(camera, cameras):
+    if camera is not None and cameras is not None:
+        raise PlsvoError("pass camera= (one ATAN camera) or cameras= (pinhole intrinsics per pair), not both")
+
+
+def _cameras_arg(cameras, data):
+    """plsvo_camera[B] for the multicam calls: `cameras` [B, 4] rows (fx, fy, cx, cy), data.cam's image size."""
+    import numpy as np
+
+    k = np.asarray(cameras, dtype=np.float64)
+    if k.shape != (data.batch, 4):
+        raise PlsvoError(f"cameras must have shape [{data.batch}, 4] (fx, fy, cx, cy per pair), got {list(k.shape)}")
+    return abi.make_cameras(k, data.cam, data.batch)
+
+
+def _frame_fx_arg(fx, batch: int):
+    import numpy as np
+
+    fxa = np.ascontiguousarray(fx, dtype=np.float64)
+    if fxa.shape != (batch,):
+        raise PlsvoError(f"fx must have shape [{batch}] (errorMultiplier2 per frame), got {list(fxa.shape)}")
+    return fxa
 
 
 def _raw_call_args(camera, raw, align_data):

@@ -211,12 +211,28 @@ __device__ __forceinline__ bool cam_in_frame(int ox, int oy, int boundary, int l
 // Camera model of the kernel, a compile-time policy.  The two models differ in world2cam (project) and cam2world only:
 // isInFrame, the Jacobian and errorMultiplier2 = |fx| are the same for both (vk::ATANCamera::errorMultiplier2 is fx_,
 // positive by validation, and AlignArgs::fx holds fx_ for the ATAN kernels).
+// PinholePerPair is the undistorted pinhole with its own fx, fy, cx, cy for every pair (a.cams[b], the multicam entry
+// points): the same expressions as PinholeCam, with the intrinsics read from pair_intrinsics() instead of AlignArgs.
 struct PinholeCam {  // vk::PinholeCamera without distortion
-  static constexpr bool kAtan = false;
+  static constexpr bool kAtan = false, kPerPair = false;
 };
 struct AtanCam {  // vk::ATANCamera, the FOV model (oracle/refdeps/vikit/atan_camera.h restates it)
-  static constexpr bool kAtan = true;
+  static constexpr bool kAtan = true, kPerPair = false;
 };
+struct PinholePerPair {  // vk::PinholeCamera without distortion, one per pair
+  static constexpr bool kAtan = false, kPerPair = true;
+};
+
+// fx, fy, cx, cy of the CTA's current pair (PinholePerPair only): static shared memory, which only the PinholePerPair
+// kernels instantiate.  The 32 bytes cost 128 per CTA (the dynamic region behind them is 128-byte aligned); the host
+// plan reads the compiled size through align_multicam_kernel_static_smem.  Thread 0 fills it from a.cams when the pair
+// starts; every use reads it back, as the pass reads ctl->dscale, so the intrinsics take no registers across the pass.
+template <class Cam>
+__device__ __forceinline__ double* pair_intrinsics() {
+  static_assert(Cam::kPerPair, "only the per-pair camera keeps its intrinsics in shared memory");
+  __shared__ double K[4];
+  return K;
+}
 
 // cam2world: the constructors of PointFeat / LineFeat derive their bearing vectors this way (src/feature.cpp:42,98-99),
 // every operation rounded on its own (Eigen: x / sqrt(x.x)).
@@ -225,7 +241,13 @@ struct AtanCam {  // vk::ATANCamera, the FOV model (oracle/refdeps/vikit/atan_ca
 //            (factor d, 1).normalized() with factor = r_d > 0.01 ? r / r_d : 1
 template <class Cam>
 __device__ __forceinline__ void cam2world(const AlignArgs& a, const double* px, double* f) {
-  double x = __ddiv_rn(__dsub_rn(px[0], a.cx), a.fx), y = __ddiv_rn(__dsub_rn(px[1], a.cy), a.fy);
+  double x, y;
+  if constexpr (Cam::kPerPair) {
+    const double* K = pair_intrinsics<Cam>();
+    x = __ddiv_rn(__dsub_rn(px[0], K[2]), K[0]), y = __ddiv_rn(__dsub_rn(px[1], K[3]), K[1]);
+  } else {
+    x = __ddiv_rn(__dsub_rn(px[0], a.cx), a.fx), y = __ddiv_rn(__dsub_rn(px[1], a.cy), a.fy);
+  }
   if constexpr (Cam::kAtan) {
     const double rd = __dsqrt_rn(__dadd_rn(__dmul_rn(x, x), __dmul_rn(y, y)));
     const double r = a.atan_s != 0.0 ? __dmul_rn(tan(__dmul_rn(rd, a.atan_s)), a.atan_tans_inv) : rd;
@@ -296,6 +318,10 @@ __device__ __forceinline__ void project(const PairCtl* ctl, const AlignArgs& a, 
     if (!(r < 0.001) && a.atan_s != 0.0) factor = __ddiv_rn(__dmul_rn(a.atan_s_inv, atan(__dmul_rn(r, a.atan_tans))), r);
     u = __dadd_rn(a.cx, __dmul_rn(a.fx, __dmul_rn(factor, un))) * ctl->dscale;
     v = __dadd_rn(a.cy, __dmul_rn(a.fy, __dmul_rn(factor, vn))) * ctl->dscale;
+  } else if constexpr (Cam::kPerPair) {
+    const double* K = pair_intrinsics<Cam>();
+    u = (K[0] * (xc * izc) + K[2]) * ctl->dscale;
+    v = (K[1] * (yc * izc) + K[3]) * ctl->dscale;
   } else {
     u = (a.fx * (xc * izc) + a.cx) * ctl->dscale;
     v = (a.fy * (yc * izc) + a.cy) * ctl->dscale;
@@ -724,6 +750,11 @@ __device__ __forceinline__ void align_pairs(const AlignArgs& a) {
       ctl->n_opq = 0;
       for (int i = 0; i < 36; ++i) ctl->H_last[i] = 0.0;
       for (int l = 0; l < PLSVO_MAX_LEVELS; ++l) ctl->iters_level[l] = 0;
+      if constexpr (Cam::kPerPair) {
+        double* K = pair_intrinsics<Cam>();
+        const plsvo_camera& cam = a.cams[b];
+        K[0] = cam.fx, K[1] = cam.fy, K[2] = cam.cx, K[3] = cam.cy;
+      }
     }
     // Host-buffer pipeline with lean inputs: pyramid levels above a.derive_from were not shipped; this CTA forms them
     // for its own pair by vk::halfSample (truncating 2x2 mean, frame_utils::createImgPyramid, src/frame.cpp:171-180)
@@ -800,7 +831,8 @@ __device__ __forceinline__ void align_pairs(const AlignArgs& a) {
         ctl->iter = 0;
         for (int i = 0; i < 7; ++i) ctl->old_model[i] = ctl->model[i];
         ctl->dscale = dscale;
-        ctl->cJ = fabs(a.fx) / (double)(1 << level);  // focal_length / 2^level (:262)
+        if constexpr (Cam::kPerPair) ctl->cJ = fabs(pair_intrinsics<Cam>()[0]) / (double)(1 << level);
+        else ctl->cJ = fabs(a.fx) / (double)(1 << level);  // focal_length / 2^level (:262)
         ctl->cJ2 = ctl->cJ * ctl->cJ;
       }
       // ---- segment sampling at this level (:285-332) ----
@@ -1357,6 +1389,11 @@ __global__ void __launch_bounds__(NT, MINB) sparse_img_align_atan_kernel(const A
   align_pairs<NT, AtanCam>(a);
 }
 
+template <int NT, int MINB>
+__global__ void __launch_bounds__(NT, MINB) sparse_img_align_multicam_kernel(const AlignArgs a) {
+  align_pairs<NT, PinholePerPair>(a);
+}
+
 }  // namespace
 
 namespace {
@@ -1457,6 +1494,54 @@ cudaError_t align_atan_kernel_launch(const AlignArgs& a, int grid, int threads, 
   if (threads == NT && min_blocks == MB) {                                   \
     sparse_img_align_atan_kernel<NT, MB><<<grid, NT, smem_bytes, s>>>(a);    \
     return cudaGetLastError();                                               \
+  }
+  PLSVO_ALIGN_VARIANTS(X)
+#undef X
+  return cudaErrorInvalidValue;
+}
+
+// the same variants with per-pair pinhole intrinsics (a.cams)
+namespace {
+template <int NT, int MINB>
+cudaError_t prepare_multicam_t(size_t smem_bytes, int* ctas_per_sm) {
+  cudaError_t e = cudaFuncSetAttribute(sparse_img_align_multicam_kernel<NT, MINB>,
+                                       cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_bytes);
+  if (e != cudaSuccess) return e;
+  e = cudaFuncSetAttribute(sparse_img_align_multicam_kernel<NT, MINB>, cudaFuncAttributePreferredSharedMemoryCarveout,
+                           cudaSharedmemCarveoutMaxShared);
+  if (e != cudaSuccess) return e;
+  return cudaOccupancyMaxActiveBlocksPerMultiprocessor(ctas_per_sm, sparse_img_align_multicam_kernel<NT, MINB>, NT,
+                                                       smem_bytes);
+}
+}  // namespace
+
+cudaError_t align_multicam_kernel_prepare(int threads, int min_blocks, size_t smem_bytes, int* ctas_per_sm) {
+#define X(NT, MB) \
+  if (threads == NT && min_blocks == MB) return prepare_multicam_t<NT, MB>(smem_bytes, ctas_per_sm);
+  PLSVO_ALIGN_VARIANTS(X)
+#undef X
+  return cudaErrorInvalidValue;
+}
+
+cudaError_t align_multicam_kernel_static_smem(int threads, int min_blocks, size_t* bytes) {
+  cudaFuncAttributes fa;
+#define X(NT, MB)                                                                           \
+  if (threads == NT && min_blocks == MB) {                                                  \
+    const cudaError_t e = cudaFuncGetAttributes(&fa, sparse_img_align_multicam_kernel<NT, MB>); \
+    *bytes = e == cudaSuccess ? fa.sharedSizeBytes : 0;                                     \
+    return e;                                                                               \
+  }
+  PLSVO_ALIGN_VARIANTS(X)
+#undef X
+  return cudaErrorInvalidValue;
+}
+
+cudaError_t align_multicam_kernel_launch(const AlignArgs& a, int grid, int threads, int min_blocks, size_t smem_bytes,
+                                         cudaStream_t s) {
+#define X(NT, MB)                                                              \
+  if (threads == NT && min_blocks == MB) {                                     \
+    sparse_img_align_multicam_kernel<NT, MB><<<grid, NT, smem_bytes, s>>>(a);  \
+    return cudaGetLastError();                                                 \
   }
   PLSVO_ALIGN_VARIANTS(X)
 #undef X

@@ -70,6 +70,8 @@ struct AlignArgs {
   // vk::ATANCamera distortion (read by the ATAN kernels only; fx, fy, cx, cy above then hold fx_, fy_, cx_, cy_):
   // s_ = d0, s_inv_ = 1/s_, tans_ = 2 tan(s_/2), tans_inv_ = 1/tans_, all zero when s_ == 0
   double atan_s, atan_s_inv, atan_tans, atan_tans_inv;
+  // [B] camera of every pair (the multicam kernels read its fx, fy, cx, cy instead of fx, fy, cx, cy above)
+  const plsvo_camera* cams;
 };
 
 // Opaque chi2 patches (16 float terms each) the alignment kernel can hold per Gauss-Newton pass: the patches whose 16
@@ -93,6 +95,16 @@ cudaError_t align_kernel_launch(const AlignArgs& a, int grid, int threads, int m
 __attribute__((weak)) cudaError_t align_atan_kernel_prepare(int threads, int min_blocks, size_t smem_bytes, int* ctas_per_sm);
 __attribute__((weak)) cudaError_t align_atan_kernel_launch(const AlignArgs& a, int grid, int threads, int min_blocks,
                                                            size_t smem_bytes, cudaStream_t s);
+// The same kernel variants with per-pair pinhole intrinsics, AlignArgs::cams (plsvo_align_multicam_batch_run).  Weak for
+// the same reason.  They hold the current pair's intrinsics in static shared memory, which the runtime reserves per CTA
+// next to the dynamic region (128 bytes on sm_90a: the 32 of the intrinsics, padded to the dynamic region's alignment);
+// align_multicam_kernel_static_smem reports the compiled size (cudaFuncAttributes::sharedSizeBytes), and the plan of
+// these kernels (and of no other) takes it into account.
+__attribute__((weak)) cudaError_t align_multicam_kernel_static_smem(int threads, int min_blocks, size_t* bytes);
+__attribute__((weak)) cudaError_t align_multicam_kernel_prepare(int threads, int min_blocks, size_t smem_bytes,
+                                                                int* ctas_per_sm);
+__attribute__((weak)) cudaError_t align_multicam_kernel_launch(const AlignArgs& a, int grid, int threads, int min_blocks,
+                                                               size_t smem_bytes, cudaStream_t s);
 
 // ---------------------------------------------------------------------------------------------
 struct PoseOptArgs {
@@ -122,9 +134,13 @@ struct PoseOptArgs {
   uint8_t* out_seg_outlier;
   int32_t* out_iters;
   int32_t* out_status;
+  const double* fx_frame;  // [B] errorMultiplier2 of every frame (read by the multicam kernel only, instead of fx)
 };
 size_t poseopt_smem_bytes(int n_pts, int n_segs);
 cudaError_t poseopt_kernel_launch(const PoseOptArgs& a, size_t smem_bytes, cudaStream_t s);
+// The same kernel with a.fx_frame (plsvo_poseopt_multicam_batch_run, plsvo_track_multicam_batch_run).  Weak, as the
+// alignment launchers above.
+__attribute__((weak)) cudaError_t poseopt_multicam_kernel_launch(const PoseOptArgs& a, size_t smem_bytes, cudaStream_t s);
 
 
 // ---------------------------------------------------------------------------------------------

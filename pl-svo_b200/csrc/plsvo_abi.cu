@@ -64,6 +64,8 @@ struct plsvo_ctx_impl {
   bool lvl_uploaded[PLSVO_MAX_LEVELS] = {false};
   bool chain = false;              // PLSVO_ALIGN_FRAME_CHAIN: one stack of B+1 frames, cur(b) = frame b+1 = ref(b+1)
   bool atan = false;               // the uploaded batch is seen through a vk::ATANCamera (the ATAN kernel variants)
+  bool multicam = false;           // every pair has its own pinhole intrinsics, aa.cams (the multicam kernel variants)
+  DevBuf d_cams;                   // plsvo_camera[B] of a multicam batch
   DevBuf d_feat;                     // every per-pair input array of the batch, at 256-byte-aligned offsets
   size_t feat_bytes = 0;
   char* h_po_out = nullptr;          // pinned staging of the pose-optimiser outputs (one D2H per download)
@@ -78,6 +80,9 @@ struct plsvo_ctx_impl {
 
   // ---- pose-opt state ----
   bool po_ready = false;
+  bool po_multicam = false;        // every frame has its own errorMultiplier2, pa.fx_frame (the multicam kernel)
+  DevBuf d_po_fx;                  // pa.fx_frame
+  std::vector<double> h_po_fx;     // the track call's |cams[b].fx|, staged for the upload
   PoseOptArgs pa;
   DevBuf y_img;  // pyramid levels
   DevBuf f_img, f_idx, f_lvl, f_border, f_ref, f_px, f_opx, f_oconv, f_dir, f_ohinv;  // align2D / align1D
@@ -357,6 +362,8 @@ int align_layout(plsvo_ctx_impl* c, const plsvo_align_batch* h) {
   // `cur_img[l] + b*stride` then simply starts one frame further into the same stack
   c->chain = (h->flags & PLSVO_ALIGN_FRAME_CHAIN) != 0;
   c->atan = false;  // the ATAN entry points set it after the upload
+  c->multicam = false;  // and so do the multicam entry points
+  a.cams = nullptr;
   a.B = h->batch, a.n_pts = h->n_pts, a.n_segs = h->n_segs;
   a.width = h->cam.width, a.height = h->cam.height;
   a.fx = h->cam.fx, a.fy = h->cam.fy, a.cx = h->cam.cx, a.cy = h->cam.cy;
@@ -804,9 +811,13 @@ int align_plan(plsvo_ctx_impl* c, const plsvo_align_params* p, AlignPlan* plan, 
       rc_last = fail(c, PLSVO_ERR_INVALID, "a segment has more than 1024 samples");
       continue;
     }
+    // static shared memory of the kernel, taken per CTA next to the dynamic plan below: the multicam kernels hold
+    // their pair's intrinsics there (with the alignment of the dynamic region behind them); the others have none
+    size_t static_smem = 0;
+    if (c->multicam) CK(align_multicam_kernel_static_smem(threads, min_blocks, &static_smem));
     // shared-memory plan: stage the current image level when the CTA still fits min_blocks times per SM next to
     // the per-pair state; bigger levels are read through L2 with the same aligned-word loads.
-    const int other = (int)align_smem_bytes(a.n_pts, a.n_segs, a.max_patches, a.max_seg_slots, 0, threads);
+    const int other = (int)(align_smem_bytes(a.n_pts, a.n_segs, a.max_patches, a.max_seg_slots, 0, threads) + static_smem);
     int img_budget = (limit + 1024) / min_blocks - 1024 - other;
     if (img_budget < 0) img_budget = 0;
     img_budget = std::min(img_budget, 96 * 1024);
@@ -819,11 +830,11 @@ int align_plan(plsvo_ctx_impl* c, const plsvo_align_params* p, AlignPlan* plan, 
       if (a.img_in_smem[l]) img_bytes = std::max(img_bytes, (int)bytes);
     }
     size_t smem = align_smem_bytes(a.n_pts, a.n_segs, a.max_patches, a.max_seg_slots, img_bytes, threads);
-    if (smem > (size_t)limit) {  // drop image staging as a last resort
+    if (smem + static_smem > (size_t)limit) {  // drop image staging as a last resort
       for (int l = 0; l < PLSVO_MAX_LEVELS; ++l) a.img_in_smem[l] = 0;
       img_bytes = 0;
       smem = align_smem_bytes(a.n_pts, a.n_segs, a.max_patches, a.max_seg_slots, 0, threads);
-      if (smem > (size_t)limit) {
+      if (smem + static_smem > (size_t)limit) {
         rc_last = fail(c, PLSVO_ERR_INVALID, "feature counts exceed the shared-memory plan");
         continue;
       }
@@ -831,13 +842,14 @@ int align_plan(plsvo_ctx_impl* c, const plsvo_align_params* p, AlignPlan* plan, 
     // the segment samples' Sxx, Sxy, Syy (formed once per level) go to shared memory when that costs neither a staged
     // level nor a resident pair, and are read through L2 otherwise
     const size_t gram_bytes = 3 * sizeof(double) * (size_t)a.max_seg_patches;
-    a.gram_in_smem = (smem + gram_bytes + 1024) * (size_t)min_blocks <= (size_t)limit + 1024 ? 1 : 0;
+    a.gram_in_smem = (smem + static_smem + gram_bytes + 1024) * (size_t)min_blocks <= (size_t)limit + 1024 ? 1 : 0;
     if (a.gram_in_smem) smem += gram_bytes;
     a.smem_img_bytes = img_bytes;
     a.rec_cap = rec_cap;
     int ctas_per_sm = 0;
-    CK(c->atan ? align_atan_kernel_prepare(threads, min_blocks, smem, &ctas_per_sm)
-               : align_kernel_prepare(threads, min_blocks, smem, &ctas_per_sm));
+    CK(c->atan       ? align_atan_kernel_prepare(threads, min_blocks, smem, &ctas_per_sm)
+       : c->multicam ? align_multicam_kernel_prepare(threads, min_blocks, smem, &ctas_per_sm)
+                     : align_kernel_prepare(threads, min_blocks, smem, &ctas_per_sm));
     if (ctas_per_sm < 1) {
       rc_last = fail(c, PLSVO_ERR_INVALID, "kernel does not fit on an SM");
       continue;
@@ -874,8 +886,9 @@ int align_launch_kernel(plsvo_ctx_impl* c, const AlignPlan& plan, cudaStream_t s
   a.gate_chunk = gate_chunk;
   const int grid = std::min(a.B, c->num_sms * plan.ctas_per_sm);
   CK(cudaMemsetAsync(a.work_counter, 0, sizeof(unsigned int), s));
-  CK(c->atan ? align_atan_kernel_launch(a, grid, plan.threads, plan.min_blocks, plan.smem, s)
-             : align_kernel_launch(a, grid, plan.threads, plan.min_blocks, plan.smem, s));
+  CK(c->atan       ? align_atan_kernel_launch(a, grid, plan.threads, plan.min_blocks, plan.smem, s)
+     : c->multicam ? align_multicam_kernel_launch(a, grid, plan.threads, plan.min_blocks, plan.smem, s)
+                   : align_kernel_launch(a, grid, plan.threads, plan.min_blocks, plan.smem, s));
   c->launches += 1;
   return PLSVO_OK;
 }
@@ -1063,6 +1076,8 @@ namespace {
 // device_T: poses already on the device (the chained call), instead of h->T_f_w
 int poseopt_upload_impl(plsvo_ctx_impl* c, const plsvo_poseopt_batch* h, const double* device_T) {
   c->po_ready = false;
+  c->po_multicam = false;  // the multicam entry points set it after the upload
+  c->pa.fx_frame = nullptr;
   if (h->batch <= 0 || h->n_pts < 0 || h->n_segs < 0) return fail(c, PLSVO_ERR_INVALID, "batch/n_pts/n_segs out of range");
   if (!h->T_f_w && !device_T) return fail(c, PLSVO_ERR_INVALID, "T_f_w missing");
   for (int b = 0; b < h->batch; ++b) {  // the counts index shared memory in the kernel
@@ -1192,7 +1207,7 @@ int plsvo_poseopt_launch(plsvo_ctx* ctx, const plsvo_poseopt_params* p) {
   if (smem > (size_t)c->smem_optin) return fail(c, PLSVO_ERR_INVALID, "feature counts exceed shared memory");
   // outputs of frames that return early keep their previous contents: clear the ones we always report
   CK(cudaMemsetAsync(static_cast<char*>(c->p_out_T.p) + c->po_zero_off, 0, c->po_zero_bytes, c->stream));
-  CK(poseopt_kernel_launch(a, smem, c->stream));
+  CK(c->po_multicam ? poseopt_multicam_kernel_launch(a, smem, c->stream) : poseopt_kernel_launch(a, smem, c->stream));
   c->launches += 1;
   return PLSVO_OK;
 }
@@ -1350,6 +1365,140 @@ int plsvo_track_atan_batch_run(plsvo_ctx* ctx, const plsvo_atan_camera* cam, con
                                const plsvo_align_result* ao, const plsvo_poseopt_result* po) {
   if (!ctx || !cam || !ab || !ap || !pb || !pp || !po) return PLSVO_ERR_INVALID;
   return settled(CTX(ctx), track_atan_body(ctx, cam, ab, ap, pb, pp, ao, po));
+}
+
+}  // extern "C"
+
+// ------------------------------------------------------------------------------------------------
+// Multicam batches: undistorted pinhole intrinsics per pair, one image size per batch
+// ------------------------------------------------------------------------------------------------
+namespace {
+
+// cams[0..B) against the batch: the size of batch->cam, finite intrinsics, fx and fy non-zero.  Nothing is queued here.
+int multicam_check(plsvo_ctx_impl* c, const plsvo_camera* cams, const plsvo_align_batch* b) {
+  if (!cams) return fail(c, PLSVO_ERR_INVALID, "cams is NULL");
+  char msg[160];
+  for (int i = 0; i < b->batch; ++i) {
+    const plsvo_camera& k = cams[i];
+    if (k.width != b->cam.width || k.height != b->cam.height) {
+      snprintf(msg, sizeof msg, "cams[%d] is %dx%d, batch->cam is %dx%d: one image size per batch", i, k.width, k.height,
+               b->cam.width, b->cam.height);
+      return fail(c, PLSVO_ERR_INVALID, msg);
+    }
+    if (!std::isfinite(k.fx) || !std::isfinite(k.fy) || !std::isfinite(k.cx) || !std::isfinite(k.cy)) {
+      snprintf(msg, sizeof msg, "cams[%d] has a non-finite fx, fy, cx or cy", i);
+      return fail(c, PLSVO_ERR_INVALID, msg);
+    }
+    if (k.fx == 0.0 || k.fy == 0.0) {
+      snprintf(msg, sizeof msg, "cams[%d].fx and fy must be non-zero", i);
+      return fail(c, PLSVO_ERR_INVALID, msg);
+    }
+  }
+  return PLSVO_OK;
+}
+
+// fx[0..B), the frames' errorMultiplier2: finite and positive.  Nothing is queued here.
+int frame_fx_check(plsvo_ctx_impl* c, const double* fx, int B) {
+  if (!fx) return fail(c, PLSVO_ERR_INVALID, "fx is NULL");
+  for (int i = 0; i < B; ++i)
+    if (!std::isfinite(fx[i]) || !(fx[i] > 0.0)) {
+      char msg[96];
+      snprintf(msg, sizeof msg, "fx[%d] must be finite and positive", i);
+      return fail(c, PLSVO_ERR_INVALID, msg);
+    }
+  return PLSVO_OK;
+}
+
+int multicam_kernels_present(plsvo_ctx_impl* c, bool align, bool poseopt) {
+  if (align && (!align_multicam_kernel_prepare || !align_multicam_kernel_launch || !align_multicam_kernel_static_smem))
+    return fail(c, PLSVO_ERR_CUDA, "this library was built without the multicam alignment kernels");
+  if (poseopt && !poseopt_multicam_kernel_launch)
+    return fail(c, PLSVO_ERR_CUDA, "this library was built without the multicam pose-optimiser kernel");
+  return PLSVO_OK;
+}
+
+// after the upload of the alignment batch: the pairs' cameras follow it on the same stream, and the multicam kernels
+// run the batch
+int multicam_select(plsvo_ctx_impl* c, const plsvo_camera* cams) {
+  CK(up(c->d_cams, cams, (size_t)c->aa.B, c->stream, &c->aa.cams));
+  c->multicam = true;
+  return PLSVO_OK;
+}
+
+// after the upload of the pose-optimiser batch: frame b's errorMultiplier2 is fx[b]
+int poseopt_fx_select(plsvo_ctx_impl* c, const double* fx) {
+  CK(up(c->d_po_fx, fx, (size_t)c->pa.B, c->stream, &c->pa.fx_frame));
+  c->po_multicam = true;
+  return PLSVO_OK;
+}
+
+}  // namespace
+
+extern "C" {
+
+static int align_multicam_body(plsvo_ctx* ctx, const plsvo_camera* cams, const plsvo_align_batch* b,
+                               const plsvo_align_params* p, const plsvo_align_result* o) {
+  plsvo_ctx_impl* c = CTX(ctx);
+  int rc = multicam_check(c, cams, b);
+  if (rc == PLSVO_OK) rc = multicam_kernels_present(c, true, false);
+  if (rc == PLSVO_OK) rc = plsvo_align_upload(ctx, b);
+  if (rc == PLSVO_OK) rc = multicam_select(c, cams);
+  if (rc == PLSVO_OK) rc = plsvo_align_launch(ctx, p);
+  if (rc == PLSVO_OK) rc = plsvo_align_download(ctx, o);
+  return rc;
+}
+
+int plsvo_align_multicam_batch_run(plsvo_ctx* ctx, const plsvo_camera* cams, const plsvo_align_batch* b,
+                                   const plsvo_align_params* p, const plsvo_align_result* o) {
+  if (!ctx || !b || !p || !o) return PLSVO_ERR_INVALID;
+  return settled(CTX(ctx), align_multicam_body(ctx, cams, b, p, o));
+}
+
+static int poseopt_multicam_body(plsvo_ctx* ctx, const double* fx, const plsvo_poseopt_batch* b,
+                                 const plsvo_poseopt_params* p, const plsvo_poseopt_result* o) {
+  plsvo_ctx_impl* c = CTX(ctx);
+  int rc = frame_fx_check(c, fx, b->batch);
+  if (rc == PLSVO_OK) rc = multicam_kernels_present(c, false, true);
+  if (rc == PLSVO_OK) rc = plsvo_poseopt_upload(ctx, b);
+  if (rc == PLSVO_OK) rc = poseopt_fx_select(c, fx);
+  if (rc == PLSVO_OK) rc = plsvo_poseopt_launch(ctx, p);
+  if (rc == PLSVO_OK) rc = plsvo_poseopt_download(ctx, o);
+  return rc;
+}
+
+int plsvo_poseopt_multicam_batch_run(plsvo_ctx* ctx, const double* fx, const plsvo_poseopt_batch* b,
+                                     const plsvo_poseopt_params* p, const plsvo_poseopt_result* o) {
+  if (!ctx || !b || !p || !o) return PLSVO_ERR_INVALID;
+  return settled(CTX(ctx), poseopt_multicam_body(ctx, fx, b, p, o));
+}
+
+static int track_multicam_body(plsvo_ctx* ctx, const plsvo_camera* cams, const plsvo_align_batch* ab,
+                               const plsvo_align_params* ap, const plsvo_poseopt_batch* pb, const plsvo_poseopt_params* pp,
+                               const plsvo_align_result* ao, const plsvo_poseopt_result* po) {
+  plsvo_ctx_impl* c = CTX(ctx);
+  int rc = multicam_check(c, cams, ab);
+  if (rc == PLSVO_OK && pb->batch != ab->batch)
+    rc = fail(c, PLSVO_ERR_INVALID, "alignment and pose-optimiser batches differ in size");
+  if (rc == PLSVO_OK) rc = multicam_kernels_present(c, true, true);
+  if (rc != PLSVO_OK) return rc;
+  // the pose optimiser of frame b reads vk::PinholeCamera::errorMultiplier2() = |fx| of pair b's camera
+  c->h_po_fx.resize((size_t)ab->batch);
+  for (int i = 0; i < ab->batch; ++i) c->h_po_fx[i] = fabs(cams[i].fx);
+  rc = plsvo_track_upload(ctx, ab, pb);
+  if (rc == PLSVO_OK) rc = multicam_select(c, cams);
+  if (rc == PLSVO_OK) rc = poseopt_fx_select(c, c->h_po_fx.data());
+  if (rc == PLSVO_OK) rc = plsvo_track_launch(ctx, ap, pp);
+  if (rc == PLSVO_OK && ao) rc = plsvo_align_download(ctx, ao);
+  if (rc == PLSVO_OK) rc = plsvo_poseopt_download(ctx, po);
+  return rc;
+}
+
+int plsvo_track_multicam_batch_run(plsvo_ctx* ctx, const plsvo_camera* cams, const plsvo_align_batch* ab,
+                                   const plsvo_align_params* ap, const plsvo_poseopt_batch* pb,
+                                   const plsvo_poseopt_params* pp, const plsvo_align_result* ao,
+                                   const plsvo_poseopt_result* po) {
+  if (!ctx || !ab || !ap || !pb || !pp || !po) return PLSVO_ERR_INVALID;
+  return settled(CTX(ctx), track_multicam_body(ctx, cams, ab, ap, pb, pp, ao, po));
 }
 
 }  // extern "C"

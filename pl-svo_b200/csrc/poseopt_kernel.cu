@@ -284,7 +284,10 @@ __device__ __forceinline__ void gn_loop(const PoseOptArgs& a, const Feat& F, PoC
 #ifndef PLSVO_PO_MINB
 #define PLSVO_PO_MINB 3  // resident CTAs per SM the register budget is compiled for (168 registers fit three)
 #endif
-__global__ void __launch_bounds__(kPoThreads, PLSVO_PO_MINB) pose_optimizer_kernel(const PoseOptArgs a) {
+// The whole kernel.  kPerFrameFx: frame b's errorMultiplier2 is a.fx_frame[b] (the multicam entry points) instead of
+// a.fx; it is the only difference between the two __global__ entry points below.
+template <bool kPerFrameFx>
+__device__ __forceinline__ void optimize_frames(const PoseOptArgs& a) {
   extern __shared__ __align__(16) unsigned char smem[];
   const int tid = threadIdx.x;
   const int n_tot = a.n_pts + a.n_segs;
@@ -310,7 +313,7 @@ __global__ void __launch_bounds__(kPoThreads, PLSVO_PO_MINB) pose_optimizer_kern
     F.seg_spos = a.seg_spos + 3 * so;
     F.seg_epos = a.seg_epos + 3 * so;
     F.seg_level = a.seg_level + so;
-    const double fx = a.fx;
+    const double fx = kPerFrameFx ? a.fx_frame[b] : a.fx;
 
     if (tid == 0) {
       const SE3q T = se3_load(a.T_f_w + (size_t)b * 7);
@@ -468,6 +471,14 @@ __global__ void __launch_bounds__(kPoThreads, PLSVO_PO_MINB) pose_optimizer_kern
   }
 }
 
+__global__ void __launch_bounds__(kPoThreads, PLSVO_PO_MINB) pose_optimizer_kernel(const PoseOptArgs a) {
+  optimize_frames<false>(a);
+}
+
+__global__ void __launch_bounds__(kPoThreads, PLSVO_PO_MINB) pose_optimizer_multicam_kernel(const PoseOptArgs a) {
+  optimize_frames<true>(a);
+}
+
 }  // namespace
 
 size_t poseopt_smem_bytes(int n_pts, int n_segs) {
@@ -479,7 +490,9 @@ size_t poseopt_smem_bytes(int n_pts, int n_segs) {
   return s;
 }
 
-cudaError_t poseopt_kernel_launch(const PoseOptArgs& a, size_t smem_bytes, cudaStream_t s) {
+namespace {
+// one launch of either entry point: at most 16 CTAs per SM, each walking its frames with a grid stride
+cudaError_t launch_frames(void (*kernel)(const PoseOptArgs), const PoseOptArgs& a, size_t smem_bytes, cudaStream_t s) {
   static int max_grid = 0;
   if (max_grid == 0) {
     int dev = 0, sms = 0;
@@ -489,11 +502,20 @@ cudaError_t poseopt_kernel_launch(const PoseOptArgs& a, size_t smem_bytes, cudaS
   }
   cudaError_t e = cudaSuccess;
   if (smem_bytes > 48 * 1024)
-    e = cudaFuncSetAttribute(pose_optimizer_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_bytes);
+    e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_bytes);
   if (e != cudaSuccess) return e;
   const int grid = a.B < max_grid ? a.B : max_grid;
-  pose_optimizer_kernel<<<grid, kPoThreads, smem_bytes, s>>>(a);
+  kernel<<<grid, kPoThreads, smem_bytes, s>>>(a);
   return cudaGetLastError();
+}
+}  // namespace
+
+cudaError_t poseopt_kernel_launch(const PoseOptArgs& a, size_t smem_bytes, cudaStream_t s) {
+  return launch_frames(pose_optimizer_kernel, a, smem_bytes, s);
+}
+
+cudaError_t poseopt_multicam_kernel_launch(const PoseOptArgs& a, size_t smem_bytes, cudaStream_t s) {
+  return launch_frames(pose_optimizer_multicam_kernel, a, smem_bytes, s);
 }
 
 }  // namespace plsvo

@@ -36,6 +36,11 @@ VGA = Camera(640, 480, 420.0, 420.0, 319.5, 239.5)
 HD720 = Camera(1280, 720, 840.0, 840.0, 639.5, 359.5)
 QVGA = Camera(320, 240, 210.0, 210.0, 159.5, 119.5)  # small case for fast CPU tests
 ODD = Camera(641, 479, 420.0, 420.0, 320.0, 239.0)  # odd sizes: no level is a multiple of 16 pixels wide
+# 640x480 cameras with the published TUM RGB-D freiburg1/2/3 intrinsics: with VGA, the four of a mixed (multicam) batch
+TUM_FR1 = Camera(640, 480, 517.3, 516.5, 318.6, 255.3)
+TUM_FR2 = Camera(640, 480, 520.9, 521.0, 325.1, 249.7)
+TUM_FR3 = Camera(640, 480, 535.4, 539.2, 320.1, 247.6)
+MULTICAM_K4 = (VGA, TUM_FR1, TUM_FR2, TUM_FR3)
 
 
 # ------------------------------------------------------------------------------------------------
@@ -513,6 +518,79 @@ def make_track_batch(cam: Camera = VGA, batch: int = 8, n_pts: int = 300, n_segs
     al = make_align_batch(cam=cam, batch=batch, n_pts=n_pts, n_segs=n_segs, seed=seed, device=device, **align_kw)
     po = make_poseopt_batch(cam=cam, batch=batch, n_pts=n_pts, n_segs=n_segs, seed=seed + 7919, T_gt=al.T_cur_w_gt)
     return al, po
+
+
+def scatter_batches(parts, index, batch: int):
+    """One batch of `batch` entries from per-group batches of the same dataclass: entry index[k][i] of the result is
+    entry i of parts[k].  Arrays of batch-first shape and dicts of them (pyramids) are scattered; the rest comes from
+    parts[0]."""
+    def merge(vals):
+        v0 = vals[0]
+        if isinstance(v0, dict):
+            return {key: merge([v[key] for v in vals]) for key in v0}
+        if isinstance(v0, np.ndarray):
+            out = np.empty((batch,) + v0.shape[1:], v0.dtype)
+            for v, idx in zip(vals, index):
+                out[idx] = v
+            return out
+        return v0
+
+    return type(parts[0])(**{f: merge([getattr(p, f) for p in parts]) for f in parts[0].__dataclass_fields__})
+
+
+def take_pairs(data, idx):
+    """Entries idx of a batch (AlignData or PoseOptData) as a batch of their own: every batch-first array attribute is
+    sliced, the two-stack pyramids (ref_pyr, cur_pyr) included; the rest (the camera, fx) is shared.  A frame chain
+    (frame_pyr set) raises ValueError: its stack has B+1 frames, so the pairs of a subset are not a chain."""
+    import copy
+
+    if getattr(data, "frame_pyr", None) is not None:
+        raise ValueError("take_pairs does not take frame chains (frame_pyr): take the pairs of the two-stack batch")
+    out = copy.copy(data)
+    B = data.batch
+    for f, v in vars(data).items():  # the dataclass fields and any array set on the instance (pt_depth, seg_sdepth, ...)
+        if isinstance(v, dict):
+            setattr(out, f, {k: np.ascontiguousarray(a[idx]) for k, a in v.items()})
+        elif isinstance(v, np.ndarray) and v.shape[:1] == (B,):
+            setattr(out, f, np.ascontiguousarray(v[idx]))
+    return out
+
+
+def multicam_cameras(cams, cam_of_pair) -> np.ndarray:
+    """[B, 4] (fx, fy, cx, cy) of every pair: row b is cams[cam_of_pair[b]] (the `cameras=` argument of the API)."""
+    k = np.array([[c.fx, c.fy, c.cx, c.cy] for c in cams], np.float64)
+    return np.ascontiguousarray(k[np.asarray(cam_of_pair)])
+
+
+def make_multicam_batch(cams, cam_of_pair, n_pts: int = 300, n_segs: int = 80, seed: int = 3000, poseopt: bool = False,
+                        **align_kw):
+    """A mixed batch from several undistorted pinhole cameras of one image size: pair b is rendered and its features are
+    lifted through cams[cam_of_pair[b]].  Each camera's pairs are one make_align_batch (make_track_batch when `poseopt`)
+    of its own, scattered to their places in the batch.  Returns (AlignData, cameras [B, 4]) — AlignData.cam is cams[0]
+    and gives only the image size — or (AlignData, PoseOptData, cameras) when `poseopt`; the pose optimiser of frame b
+    then takes errorMultiplier2 = cameras[b, 0]."""
+    cam_of_pair = np.asarray(cam_of_pair)
+    if len({(c.width, c.height) for c in cams}) != 1:
+        raise ValueError("every camera of a multicam batch has the same image size")
+    groups = [np.flatnonzero(cam_of_pair == k) for k in range(len(cams))]
+    used = [k for k in range(len(cams)) if len(groups[k])]
+    al_parts, po_parts = [], []
+    for k in used:
+        kw = dict(cam=cams[k], batch=len(groups[k]), n_pts=n_pts, n_segs=n_segs, seed=seed + 104729 * k, **align_kw)
+        if poseopt:
+            al, po = make_track_batch(**kw)
+            po_parts.append(po)
+        else:
+            al = make_align_batch(**kw)
+        al_parts.append(al)
+    B = len(cam_of_pair)
+    index = [groups[k] for k in used]
+    al = scatter_batches(al_parts, index, B)
+    al.cam = cams[0]
+    cameras = multicam_cameras(cams, cam_of_pair)
+    if not poseopt:
+        return al, cameras
+    return al, scatter_batches(po_parts, index, B), cameras
 
 
 def make_sequence(cam: Camera = VGA, n_seq: int = 4, n_frames: int = 20, n_pts: int = 300, n_segs: int = 80, seed: int = 1000,
