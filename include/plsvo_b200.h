@@ -296,7 +296,8 @@ typedef struct plsvo_undistort_batch {
 int plsvo_undistort_batch_run(plsvo_ctx* ctx, const plsvo_undistort_batch* in, const plsvo_pyramid_result* out);
 
 /* device time (CUDA events) of the map build the last plsvo_undistort_batch_run call made, or -1 in *ms when that
- * call reused the context's cached map or needed none (d0 = 0).  plsvo_last_kernel_ms never includes it. */
+ * call reused the context's cached map or needed none (d0 = 0).  After a raw multicam call: the time of all the map
+ * builds it made.  plsvo_last_kernel_ms never includes it. */
 int plsvo_last_map_build_ms(plsvo_ctx* ctx, float* ms);
 
 /* ------------------------------------------------------------------------------------------
@@ -338,6 +339,47 @@ int plsvo_track_raw_batch_run(plsvo_ctx* ctx, const plsvo_raw_frames* raw, const
                               const plsvo_align_params* al_params, const plsvo_poseopt_batch* po_batch,
                               const plsvo_poseopt_params* po_params, const plsvo_align_result* al_out,
                               const plsvo_poseopt_result* po_out, const plsvo_pyramid_result* rect_out);
+
+/* ------------------------------------------------------------------------------------------
+ * Raw frames from differently calibrated distorted cameras in one batch: the raw-frame calls above with the multicam
+ * calls' per-pair intrinsics below.  cams[k] are distorted vk::PinholeCamera arguments (d0..d4 as for
+ * plsvo_undistort_batch), all of batch->cam's image size; both frames of pair b are rectified with cams[cam_of_pair[b]],
+ * and the pair is then aligned with that camera's fx, fy, cx, cy as its undistorted intrinsics (run_pipeline builds both
+ * cameras from the same values).  In the track call frame b's errorMultiplier2 is |fx| of that camera.  Of batch->cam
+ * only width and height are used.
+ * - Pair b's outputs are byte for byte those of plsvo_align_raw_batch_run / plsvo_track_raw_batch_run on that pair with
+ *   raw->cam = cams[cam_of_pair[b]], batch->cam carrying its intrinsics, and the same kernel variant.
+ * - rect_out as for the raw calls: every non-NULL level, the B reference frames followed by the B current frames, each
+ *   rectified with its own camera (plsvo_undistort_batch_run of that frame).  Cameras with fabs(d0) <= 1e-7 copy the frame
+ *   and may be mixed with distorted ones.
+ * - The maps are built on the device once per camera and kept in a cache of the context separate from the one-camera
+ *   cache of plsvo_undistort_batch_run and the raw calls: after a call it holds the maps of exactly the distorted cameras
+ *   that call referenced (equal cameras, byte for byte, share one map).  plsvo_last_map_build_ms reports the device time
+ *   of the builds the call made, or -1 when it made none.
+ * - n_cams < 1, NULL cams or cam_of_pair, an index outside [0, n_cams), a camera whose size differs from batch->cam or
+ *   whose parameters plsvo_undistort_batch_run rejects, PLSVO_ALIGN_FRAME_CHAIN (a chained frame belongs to two pairs),
+ *   and everything the raw calls reject return PLSVO_ERR_INVALID before anything is queued.  A library built without the
+ *   multicam kernels returns PLSVO_ERR_CUDA.  The calls always run upload -> launch -> download and have finished with
+ *   the caller's arrays when they return, whatever they return.
+ * - Out of scope: per-pair image sizes, ATAN cameras, frame chains, the arrival-gated path.
+ * ---------------------------------------------------------------------------------------- */
+typedef struct plsvo_raw_multicam_frames {
+  int32_t n_cams, reserved;
+  const plsvo_pinhole_camera* cams; /* [n_cams] distorted cameras (d0..d4 as plsvo_undistort_batch), one image size */
+  const int32_t* cam_of_pair;       /* [B] index into cams: the camera of both frames of pair b */
+  const uint8_t* ref_raw;           /* [B] raw frames */
+  const uint8_t* cur_raw;           /* [B] raw frames */
+  size_t pitch, stride;             /* host layout of both stacks, as plsvo_raw_frames */
+} plsvo_raw_multicam_frames;
+
+int plsvo_align_raw_multicam_batch_run(plsvo_ctx* ctx, const plsvo_raw_multicam_frames* raw, const plsvo_align_batch* batch,
+                                       const plsvo_align_params* params, const plsvo_align_result* out,
+                                       const plsvo_pyramid_result* rect_out);
+int plsvo_track_raw_multicam_batch_run(plsvo_ctx* ctx, const plsvo_raw_multicam_frames* raw,
+                                       const plsvo_align_batch* al_batch, const plsvo_align_params* al_params,
+                                       const plsvo_poseopt_batch* po_batch, const plsvo_poseopt_params* po_params,
+                                       const plsvo_align_result* al_out, const plsvo_poseopt_result* po_out,
+                                       const plsvo_pyramid_result* rect_out);
 
 /* ------------------------------------------------------------------------------------------
  * Alignment and tracking of frames from an ATAN (FOV) camera: vk::ATANCamera, the model app/run_pipeline.cpp builds when
@@ -393,8 +435,8 @@ int plsvo_track_atan_batch_run(plsvo_ctx* ctx, const plsvo_atan_camera* cam, con
  * - The multicam kernels keep the pair's intrinsics in 128 bytes of shared memory per CTA.  A batch whose shared-memory
  *   plan lies within that of the limit is planned for the next kernel variant, as any batch that does not fit; with no
  *   variant left, or PLSVO_VARIANT pinned, it returns PLSVO_ERR_INVALID (DESIGN.md §4.11).
- * - Out of scope: per-pair image sizes, per-pair ATAN cameras, raw frames (plsvo_*_raw_batch_run), the arrival-gated
- *   streamed path, separate upload / launch / download legs, dist.align_sharded, the next-row kernels (direct matching,
+ * - Raw frames: plsvo_*_raw_multicam_batch_run above.
+ * - Out of scope: per-pair image sizes, per-pair ATAN cameras, the arrival-gated streamed path, separate upload / launch / download legs, dist.align_sharded, the next-row kernels (direct matching,
  *   seed updates, structure optimisation) and the drop-in shim (one frame per call, nothing to batch).
  * ---------------------------------------------------------------------------------------- */
 int plsvo_align_multicam_batch_run(plsvo_ctx* ctx, const plsvo_camera* cams /* [B] */, const plsvo_align_batch* batch,

@@ -166,6 +166,14 @@ class RawFrames(C.Structure):
     _fields_ = [("cam", PinholeCamera), ("ref_raw", _u8p), ("cur_raw", _u8p), ("pitch", C.c_size_t), ("stride", C.c_size_t)]
 
 
+class RawMulticamFrames(C.Structure):
+    """plsvo_raw_multicam_frames: the distorted cameras, the camera of every pair and the raw frame stacks of
+    plsvo_align_raw_multicam_batch_run / plsvo_track_raw_multicam_batch_run."""
+    _fields_ = [("n_cams", C.c_int32), ("reserved", C.c_int32), ("cams", C.POINTER(PinholeCamera)),
+                ("cam_of_pair", C.POINTER(C.c_int32)), ("ref_raw", _u8p), ("cur_raw", _u8p), ("pitch", C.c_size_t),
+                ("stride", C.c_size_t)]
+
+
 class AtanCamera(C.Structure):
     """plsvo_atan_camera: the vk::ATANCamera constructor arguments (fx, fy, cx, cy normalised by the image size)."""
     _fields_ = [("width", C.c_int32), ("height", C.c_int32), ("fx", C.c_double), ("fy", C.c_double), ("cx", C.c_double),
@@ -202,6 +210,23 @@ def make_raw_frames(cam: PinholeCamera, raw, batch: int):
     r = RawFrames(cam, stacks[0].ctypes.data_as(_u8p), None if chain else stacks[1].ctypes.data_as(_u8p),
                   stacks[0].strides[1], stacks[0].strides[0])
     return r, chain, stacks
+
+
+def make_raw_multicam_frames(cams, cam_of_pair, raw, batch: int):
+    """plsvo_raw_multicam_frames for `batch` pairs: cams, a sequence of PinholeCamera structs of one image size;
+    cam_of_pair, the index of every pair's camera; raw, a (ref, cur) pair of u8 [B,H,W] stacks with the same strides
+    (rows may be padded).  Returns (struct, keepalive)."""
+    if not isinstance(raw, (tuple, list)):
+        raise ValueError("raw multicam frames: a (ref, cur) pair of [B,H,W] stacks (frame chains are not supported)")
+    if len(cams) < 1:
+        raise ValueError("raw multicam frames: at least one camera")
+    k = np.ascontiguousarray(cam_of_pair, dtype=np.int32)
+    if k.shape != (batch,):
+        raise ValueError(f"cam_of_pair must have shape [{batch}], got {list(k.shape)}")
+    arr = (PinholeCamera * len(cams))(*cams)
+    r, _, stacks = make_raw_frames(cams[0], raw, batch)
+    m = RawMulticamFrames(len(cams), 0, arr, k.ctypes.data_as(C.POINTER(C.c_int32)), r.ref_raw, r.cur_raw, r.pitch, r.stride)
+    return m, (arr, k, stacks)
 
 
 def pyramid_levels(B: int, H: int, W: int, n_levels: int):
@@ -485,6 +510,11 @@ ABI_SYMBOLS = [
                                             _P(PyramidResult)]),
     ("plsvo_track_raw_batch_run", C.c_int, [C.c_void_p, _P(RawFrames), _P(AlignBatch), _P(AlignParams), _P(PoseOptBatch),
                                             _P(PoseOptParams), _P(AlignResult), _P(PoseOptResult), _P(PyramidResult)]),
+    ("plsvo_align_raw_multicam_batch_run", C.c_int, [C.c_void_p, _P(RawMulticamFrames), _P(AlignBatch), _P(AlignParams),
+                                                     _P(AlignResult), _P(PyramidResult)]),
+    ("plsvo_track_raw_multicam_batch_run", C.c_int, [C.c_void_p, _P(RawMulticamFrames), _P(AlignBatch), _P(AlignParams),
+                                                     _P(PoseOptBatch), _P(PoseOptParams), _P(AlignResult), _P(PoseOptResult),
+                                                     _P(PyramidResult)]),
     ("plsvo_align_atan_batch_run", C.c_int, [C.c_void_p, _P(AtanCamera), _P(AlignBatch), _P(AlignParams), _P(AlignResult)]),
     ("plsvo_track_atan_batch_run", C.c_int, [C.c_void_p, _P(AtanCamera), _P(AlignBatch), _P(AlignParams), _P(PoseOptBatch),
                                              _P(PoseOptParams), _P(AlignResult), _P(PoseOptResult)]),

@@ -144,19 +144,24 @@ class SparseImgAlign:
         self.last = out
         return out
 
-    def run_raw(self, camera: "PinholeCamera", raw, data, rect_levels=None):
+    def run_raw(self, camera: "PinholeCamera", raw, data, rect_levels=None, cam_of_pair=None):
         """run() on raw (distorted) frames: each frame is rectified with `camera` (PinholeCamera.undistortImage) and
         half-sampled on the device, and the pyramid never leaves it.  raw: a [B+1,H,W] frame chain, or a (ref, cur) pair
         of [B,H,W] stacks; rows may be padded.  data describes features, poses and the undistorted camera as for run()
         (its images are ignored).  Results are byte-identical to undistortImage followed by the plain host-buffer run().
         rect_levels: levels to bring back as well; returns (AlignOut, {level: [n_frames, H>>l, W>>l]}) then, the frames
-        in stack order (the chain, or the reference frames followed by the current ones)."""
-        rf, batch, keep = _raw_call_args(camera, raw, data)
-        levels, r = _rect_outputs(camera, rf, data.batch, rect_levels)
+        in stack order (the chain, or the reference frames followed by the current ones).
+        cam_of_pair: [B] indices into `camera`, then a sequence of PinholeCamera of data.cam's image size, when the
+        pairs come from differently calibrated lenses (plsvo_align_raw_multicam_batch_run): pair b is rectified with
+        camera[cam_of_pair[b]] and aligned with its fx, fy, cx, cy; data.cam gives only the image size.  raw must then
+        be a (ref, cur) pair of stacks."""
+        rf, batch, keep = _raw_call_args(camera, raw, data, cam_of_pair)
+        levels, r = _rect_outputs(camera if cam_of_pair is None else camera[0], rf, data.batch, rect_levels)
         out = abi.AlignOut(data.batch, data.n_segs)
-        self.ctx.check(self.ctx.lib.plsvo_align_raw_batch_run(self.ctx.handle, C.byref(rf), C.byref(batch), C.byref(self.params),
-                                                              C.byref(out.struct), C.byref(r) if r is not None else None),
-                       "plsvo_align_raw_batch_run")
+        fn, name = ((self.ctx.lib.plsvo_align_raw_batch_run, "plsvo_align_raw_batch_run") if cam_of_pair is None else
+                    (self.ctx.lib.plsvo_align_raw_multicam_batch_run, "plsvo_align_raw_multicam_batch_run"))
+        self.ctx.check(fn(self.ctx.handle, C.byref(rf), C.byref(batch), C.byref(self.params), C.byref(out.struct),
+                          C.byref(r) if r is not None else None), name)
         self.last = out
         return out if rect_levels is None else (out, levels)
 
@@ -253,9 +258,21 @@ def _frame_fx_arg(fx, batch: int):
     return fxa
 
 
-def _raw_call_args(camera, raw, align_data):
-    """plsvo_raw_frames and an image-free plsvo_align_batch (flags from the layout of `raw`) for the raw-frame calls."""
-    rf, chain, keep_r = abi.make_raw_frames(camera.struct, raw, align_data.batch)
+def _raw_call_args(camera, raw, align_data, cam_of_pair=None):
+    """plsvo_raw_frames (plsvo_raw_multicam_frames when cam_of_pair is given, `camera` then a sequence of PinholeCamera)
+    and an image-free plsvo_align_batch (flags from the layout of `raw`) for the raw-frame calls."""
+    if cam_of_pair is None:
+        rf, chain, keep_r = abi.make_raw_frames(camera.struct, raw, align_data.batch)
+    else:
+        try:
+            structs = [c.struct for c in camera]
+        except (TypeError, AttributeError):
+            raise PlsvoError("with cam_of_pair, camera must be a sequence of PinholeCamera") from None
+        try:
+            rf, keep_r = abi.make_raw_multicam_frames(structs, cam_of_pair, raw, align_data.batch)
+        except ValueError as e:
+            raise PlsvoError(str(e)) from None
+        chain = False
     batch, keep_a = abi.make_align_batch(align_data)
     for l in range(abi.MAX_LEVELS):
         batch.ref_img[l] = batch.cur_img[l] = None
@@ -283,22 +300,25 @@ def _rect_outputs(camera, rf, B: int, rect_levels):
 
 def track_raw(camera, raw, align_data, poseopt_data, max_level: int = 4, min_level: int = 2, n_iter: int = 30,
               reproj_thresh: float = 2.0, po_n_iter: int = 10, po_n_iter_ref: int | None = None, chained: bool = True,
-              ctx: Context | None = None, rect_levels=None):
-    """track() on raw (distorted) frames, rectified with `camera` on the device (see SparseImgAlign.run_raw for `raw` and
-    `rect_levels`).  Returns (AlignOut, PoseOptOut), plus the dict of rectified levels when rect_levels is given."""
+              ctx: Context | None = None, rect_levels=None, cam_of_pair=None):
+    """track() on raw (distorted) frames, rectified with `camera` on the device (see SparseImgAlign.run_raw for `raw`,
+    `rect_levels` and `cam_of_pair`; with cam_of_pair, frame b's errorMultiplier2 is |fx| of its camera and
+    poseopt_data.fx is not used).  Returns (AlignOut, PoseOptOut), plus the dict of rectified levels when rect_levels
+    is given."""
     ctx = ctx or default_context()
     ap = abi.align_params(max_level, min_level, n_iter)
     pp = abi.poseopt_params(reproj_thresh, po_n_iter, -1 if po_n_iter_ref is None else po_n_iter_ref)
-    rf, ab, keep_a = _raw_call_args(camera, raw, align_data)
+    rf, ab, keep_a = _raw_call_args(camera, raw, align_data, cam_of_pair)
     pb, keep_p = abi.make_poseopt_batch(poseopt_data)
     if chained:
         pb.T_f_w = abi._f64p()
-    levels, r = _rect_outputs(camera, rf, align_data.batch, rect_levels)
+    levels, r = _rect_outputs(camera if cam_of_pair is None else camera[0], rf, align_data.batch, rect_levels)
     ao = abi.AlignOut(align_data.batch, align_data.n_segs)
     po = abi.PoseOptOut(poseopt_data.batch, poseopt_data.n_pts, poseopt_data.n_segs)
-    ctx.check(ctx.lib.plsvo_track_raw_batch_run(ctx.handle, C.byref(rf), C.byref(ab), C.byref(ap), C.byref(pb), C.byref(pp),
-                                                C.byref(ao.struct), C.byref(po.struct), C.byref(r) if r is not None else None),
-              "plsvo_track_raw_batch_run")
+    fn, name = ((ctx.lib.plsvo_track_raw_batch_run, "plsvo_track_raw_batch_run") if cam_of_pair is None else
+                (ctx.lib.plsvo_track_raw_multicam_batch_run, "plsvo_track_raw_multicam_batch_run"))
+    ctx.check(fn(ctx.handle, C.byref(rf), C.byref(ab), C.byref(ap), C.byref(pb), C.byref(pp), C.byref(ao.struct), C.byref(po.struct),
+                 C.byref(r) if r is not None else None), name)
     return (ao, po) if rect_levels is None else (ao, po, levels)
 
 

@@ -194,6 +194,15 @@ struct RawPyramidArgs {
   size_t stride[PLSVO_MAX_LEVELS];
 };
 __attribute__((weak)) cudaError_t undistort_pyramid_launch(const RawPyramidArgs& a, int num_sms, cudaStream_t s);
+struct RawVisit {           // one frame of a multicam raw batch and the map it is rectified with
+  const short2* map1;       // its camera's map ([height][map_pitch], as RawPyramidArgs::map1), or NULL: copy the frame
+  const uint16_t* map2;
+  int32_t frame, reserved;  // index into src and every level
+};
+// The same kernel for frames of several cameras (plsvo_*_raw_multicam_batch_run): visit[0..a.B) lists every frame once,
+// in the order the CTAs' frame runs take them, each with its camera's map (a.map1 / a.map2 are not read).
+__attribute__((weak)) cudaError_t undistort_pyramid_multicam_launch(const RawPyramidArgs& a, const RawVisit* visit, int num_sms,
+                                                                    cudaStream_t s);
 
 
 // ---------------------------------------------------------------------------------------------

@@ -10,6 +10,7 @@
 
 #include <algorithm>
 #include <array>
+#include <memory>
 #include <string>
 #include <thread>
 #include <vector>
@@ -97,6 +98,15 @@ struct plsvo_ctx_impl {
   bool u_map_ok = false;
   bool u_map_built = false;  // the last undistort call built the map (timed by u_map_ev)
   cudaEvent_t u_map_ev[2] = {nullptr, nullptr};
+  // the raw multicam calls' maps: one per distinct distorted camera the last such call referenced
+  struct CamMap {
+    plsvo_pinhole_camera cam;
+    DevBuf map1, map2;
+  };
+  std::vector<std::unique_ptr<CamMap>> mc_maps;
+  std::vector<plsvo_camera> h_mc_cams;  // plsvo_camera[B] of a raw multicam call, staged for multicam_select
+  std::vector<RawVisit> h_visit;        // the frames of a raw multicam call in camera-grouped order, with their maps
+  DevBuf d_visit;
   DevBuf p_out_T;  // every pose-optimiser output, one block
 };
 
@@ -1931,29 +1941,44 @@ extern "C" int plsvo_pyramid_batch_run(plsvo_ctx* ctx, const plsvo_pyramid_batch
 }
 
 namespace {
+// entries per map row: whole remap tiles
+int map_pitch_of(int width) { return (width + kRemapTileW - 1) / kRemapTileW * kRemapTileW; }
+
+// The two halves of a map build into map1 / map2 (grown as needed): the buffers with their row padding cleared, then
+// the map kernel.  The callers time the kernels alone (plsvo_last_map_build_ms).
+int map_alloc(plsvo_ctx_impl* c, const plsvo_pinhole_camera& cam, DevBuf& map1, DevBuf& map2, cudaStream_t s) {
+  const size_t n = (size_t)cam.height * map_pitch_of(cam.width);
+  CK(ensure(map1, n * sizeof(short2)));
+  CK(ensure(map2, n * sizeof(uint16_t)));
+  CK(cudaMemsetAsync(map1.p, 0, n * sizeof(short2), s));  // the row padding: read by whole-tile loads, never used
+  CK(cudaMemsetAsync(map2.p, 0, n * sizeof(uint16_t), s));
+  return PLSVO_OK;
+}
+
+int map_launch(plsvo_ctx_impl* c, const plsvo_pinhole_camera& cam, DevBuf& map1, DevBuf& map2, cudaStream_t s) {
+  UndistortMapArgs m;
+  m.width = cam.width, m.height = cam.height, m.map_pitch = map_pitch_of(cam.width);
+  m.fx = (float)cam.fx, m.fy = (float)cam.fy, m.cx = (float)cam.cx, m.cy = (float)cam.cy;
+  m.k1 = (float)cam.d[0], m.k2 = (float)cam.d[1], m.p1 = (float)cam.d[2], m.p2 = (float)cam.d[3], m.k3 = (float)cam.d[4];
+  m.map1 = static_cast<short2*>(map1.p);
+  m.map2 = static_cast<uint16_t*>(map2.p);
+  CK(undistort_map_launch(m, s));
+  c->launches += 1;
+  return PLSVO_OK;
+}
+
 // The CV_16SC2 map of a distorted camera, built on the device when the context's cached map is of another camera (or
 // image size).  Sets u_map_built when it builds one (plsvo_last_map_build_ms).
 int undistort_map_ensure(plsvo_ctx_impl* c, const plsvo_pinhole_camera& cam, cudaStream_t s) {
   if (c->u_map_ok && memcmp(&c->u_cam, &cam, sizeof cam) == 0) return PLSVO_OK;
-  const int W = cam.width, H = cam.height;
   c->u_map_ok = false;
-  const int mp = (W + kRemapTileW - 1) / kRemapTileW * kRemapTileW;
-  const size_t n = (size_t)H * mp;
-  CK(ensure(c->u_map1, n * sizeof(short2)));
-  CK(ensure(c->u_map2, n * sizeof(uint16_t)));
-  CK(cudaMemsetAsync(c->u_map1.p, 0, n * sizeof(short2), s));  // the row padding: read by whole-tile loads, never used
-  CK(cudaMemsetAsync(c->u_map2.p, 0, n * sizeof(uint16_t), s));
-  UndistortMapArgs m;
-  m.width = W, m.height = H, m.map_pitch = mp;
-  m.fx = (float)cam.fx, m.fy = (float)cam.fy, m.cx = (float)cam.cx, m.cy = (float)cam.cy;
-  m.k1 = (float)cam.d[0], m.k2 = (float)cam.d[1], m.p1 = (float)cam.d[2], m.p2 = (float)cam.d[3], m.k3 = (float)cam.d[4];
-  m.map1 = static_cast<short2*>(c->u_map1.p);
-  m.map2 = static_cast<uint16_t*>(c->u_map2.p);
+  int rc = map_alloc(c, cam, c->u_map1, c->u_map2, s);
+  if (rc != PLSVO_OK) return rc;
   CK(record_event(c->u_map_ev[0], s));
-  CK(undistort_map_launch(m, s));
+  rc = map_launch(c, cam, c->u_map1, c->u_map2, s);
+  if (rc != PLSVO_OK) return rc;
   CK(record_event(c->u_map_ev[1], s));
-  c->launches += 1;
-  c->u_cam = cam, c->u_map_pitch = mp, c->u_map_ok = true, c->u_map_built = true;
+  c->u_cam = cam, c->u_map_pitch = map_pitch_of(cam.width), c->u_map_ok = true, c->u_map_built = true;
   return PLSVO_OK;
 }
 
@@ -2064,29 +2089,145 @@ extern "C" int plsvo_last_map_build_ms(plsvo_ctx* ctx, float* ms) {
   return PLSVO_OK;
 }
 
-// plsvo_align_raw_batch_run / plsvo_track_raw_batch_run (pb == NULL: alignment only): raw frames up, the camera's map
-// (cached), one undistort_pyramid_kernel over every frame storing the levels alignment reads and those rect_out asks for,
-// straight into the device layout of the alignment batch, then the alignment (and pose-optimiser) kernels as the plain
-// upload -> launch -> download sequence runs them.  The arrival-gated streamed path is not taken.
-static int raw_run_body(plsvo_ctx* ctx, const plsvo_raw_frames* raw, const plsvo_align_batch* ab, const plsvo_align_params* ap,
+namespace {
+// The raw frames of one raw call: one camera for every pair (plsvo_raw_frames), or cams[cam_of_pair[b]] for pair b
+// (multicam: plsvo_raw_multicam_frames).
+struct RawInput {
+  bool multicam;
+  const plsvo_pinhole_camera* cams;
+  int n_cams;
+  const int32_t* cam_of_pair;
+  const uint8_t* ref_raw;
+  const uint8_t* cur_raw;
+  size_t pitch, stride;
+};
+
+// The cameras of a multicam raw call against the batch.  Nothing is queued here.
+int raw_multicam_check(plsvo_ctx_impl* c, const RawInput& in, const plsvo_align_batch* ab) {
+  if (in.n_cams < 1 || !in.cams || !in.cam_of_pair)
+    return fail(c, PLSVO_ERR_INVALID, "raw multicam frames: n_cams must be at least 1, cams and cam_of_pair non-NULL");
+  if (ab->flags & PLSVO_ALIGN_FRAME_CHAIN)
+    return fail(c, PLSVO_ERR_INVALID, "raw multicam frames: PLSVO_ALIGN_FRAME_CHAIN is not supported (a chained frame belongs to two pairs)");
+  char msg[160];
+  for (int k = 0; k < in.n_cams; ++k) {
+    const plsvo_pinhole_camera& cam = in.cams[k];
+    if (cam.width != ab->cam.width || cam.height != ab->cam.height) {
+      snprintf(msg, sizeof msg, "raw multicam frames: cams[%d] is %dx%d, batch->cam is %dx%d: one image size per batch", k, cam.width,
+               cam.height, ab->cam.width, ab->cam.height);
+      return fail(c, PLSVO_ERR_INVALID, msg);
+    }
+    snprintf(msg, sizeof msg, "raw multicam frames: cams[%d]", k);
+    if (check_pinhole_params(c, cam, msg) != PLSVO_OK) return PLSVO_ERR_INVALID;
+  }
+  for (int b = 0; b < ab->batch; ++b)
+    if (in.cam_of_pair[b] < 0 || in.cam_of_pair[b] >= in.n_cams) {
+      snprintf(msg, sizeof msg, "raw multicam frames: cam_of_pair[%d] = %d is outside [0, %d)", b, in.cam_of_pair[b], in.n_cams);
+      return fail(c, PLSVO_ERR_INVALID, msg);
+    }
+  return PLSVO_OK;
+}
+
+// PinholeCamera's distortion_ flag: without it undistortImage is a copy
+bool distorted(const plsvo_pinhole_camera& cam) { return fabs(cam.d[0]) > 0.0000001; }
+
+// The maps of a multicam raw call and the order its frames are visited in (c->h_visit).  The cache keeps the maps of
+// the distinct distorted cameras the pairs reference, byte-equal cameras sharing one, and drops the others; a camera
+// already cached is not rebuilt.  Frames [0, B) are the reference frames of the pairs, [B, 2B) the current ones.  The
+// visit order is a counting sort of the frames by map (copied frames last), ascending frame index within a map.
+int raw_multicam_maps(plsvo_ctx_impl* c, const RawInput& in, int B, cudaStream_t s) {
+  using CamMap = plsvo_ctx_impl::CamMap;
+  std::vector<int> slot_of_cam((size_t)in.n_cams, -2);  // -2: not referenced, -1: no distortion, else its map
+  for (int b = 0; b < B; ++b) slot_of_cam[in.cam_of_pair[b]] = -1;
+  std::vector<const plsvo_pinhole_camera*> slot_cam;  // the camera of every map
+  auto same_as = [](const plsvo_pinhole_camera& cam) {
+    return [&cam](const plsvo_pinhole_camera& other) { return memcmp(&other, &cam, sizeof cam) == 0; };
+  };
+  for (int k = 0; k < in.n_cams; ++k) {
+    if (slot_of_cam[k] == -2 || !distorted(in.cams[k])) continue;
+    const auto same = same_as(in.cams[k]);
+    auto it = std::find_if(slot_cam.begin(), slot_cam.end(), [&](const plsvo_pinhole_camera* m) { return same(*m); });
+    if (it == slot_cam.end()) it = slot_cam.insert(it, &in.cams[k]);
+    slot_of_cam[k] = (int)(it - slot_cam.begin());
+  }
+  // cached maps are taken over; missing ones reuse the buffers of cached maps no longer referenced, the rest are freed
+  std::vector<std::unique_ptr<CamMap>> old = std::move(c->mc_maps), maps(slot_cam.size());
+  std::vector<size_t> missing;
+  for (size_t m = 0; m < slot_cam.size(); ++m) {
+    const auto same = same_as(*slot_cam[m]);
+    auto hit = std::find_if(old.begin(), old.end(), [&](const std::unique_ptr<CamMap>& e) { return e && same(e->cam); });
+    if (hit != old.end()) maps[m] = std::move(*hit);
+    else missing.push_back(m);
+  }
+  for (size_t m : missing) {
+    auto spare = std::find_if(old.begin(), old.end(), [](const std::unique_ptr<CamMap>& e) { return e != nullptr; });
+    maps[m] = spare != old.end() ? std::move(*spare) : std::make_unique<CamMap>();
+    memset(&maps[m]->cam, 0, sizeof maps[m]->cam);  // no camera's map until it is built
+  }
+  old.clear();
+  c->mc_maps = std::move(maps);
+  for (size_t m : missing) {
+    const int rc = map_alloc(c, *slot_cam[m], c->mc_maps[m]->map1, c->mc_maps[m]->map2, s);
+    if (rc != PLSVO_OK) return rc;
+  }
+  if (!missing.empty()) {
+    CK(record_event(c->u_map_ev[0], s));
+    for (size_t m : missing) {
+      const int rc = map_launch(c, *slot_cam[m], c->mc_maps[m]->map1, c->mc_maps[m]->map2, s);
+      if (rc != PLSVO_OK) return rc;
+      c->mc_maps[m]->cam = *slot_cam[m];
+    }
+    CK(record_event(c->u_map_ev[1], s));
+    c->u_map_built = true;
+  }
+  const int n_maps = (int)c->mc_maps.size();
+  auto key = [&](int f) {
+    const int slot = slot_of_cam[in.cam_of_pair[f < B ? f : f - B]];
+    return slot < 0 ? n_maps : slot;
+  };
+  std::vector<int> start((size_t)n_maps + 2, 0);
+  for (int f = 0; f < 2 * B; ++f) start[key(f) + 1] += 1;
+  for (int k = 0; k <= n_maps; ++k) start[k + 1] += start[k];
+  c->h_visit.resize((size_t)2 * B);
+  for (int f = 0; f < 2 * B; ++f) {
+    const int k = key(f);
+    RawVisit& v = c->h_visit[start[k]++];
+    v.map1 = k < n_maps ? static_cast<const short2*>(c->mc_maps[k]->map1.p) : nullptr;
+    v.map2 = k < n_maps ? static_cast<const uint16_t*>(c->mc_maps[k]->map2.p) : nullptr;
+    v.frame = f, v.reserved = 0;
+  }
+  return PLSVO_OK;
+}
+}  // namespace
+
+// plsvo_align_raw_batch_run / plsvo_track_raw_batch_run and their multicam forms (pb == NULL: alignment only): raw
+// frames up, the cameras' maps (cached), one rectify + pyramid kernel over every frame storing the levels alignment reads
+// and those rect_out asks for, straight into the device layout of the alignment batch, then the alignment (and
+// pose-optimiser) kernels as the plain upload -> launch -> download sequence runs them, with the multicam kernels and
+// the pairs' own intrinsics for a multicam call.  The arrival-gated streamed path is not taken.
+static int raw_run_body(plsvo_ctx* ctx, const RawInput& in, const plsvo_align_batch* ab, const plsvo_align_params* ap,
                         const plsvo_poseopt_batch* pb, const plsvo_poseopt_params* pp, const plsvo_align_result* ao,
                         const plsvo_poseopt_result* po, const plsvo_pyramid_result* rect) {
   plsvo_ctx_impl* c = CTX(ctx);
   c->u_map_built = false;
-  const plsvo_pinhole_camera& cam = raw->cam;
-  const int W = cam.width, H = cam.height;
+  const bool multicam = in.multicam;
+  const int W = multicam ? ab->cam.width : in.cams[0].width, H = multicam ? ab->cam.height : in.cams[0].height;
   if (W <= 0 || H <= 0) return fail(c, PLSVO_ERR_INVALID, "raw frames: width and height must be positive");
-  if (check_pinhole_params(c, cam, "raw-frame camera") != PLSVO_OK) return PLSVO_ERR_INVALID;
-  if (ab->cam.width != W || ab->cam.height != H || ab->cam.fx != cam.fx || ab->cam.fy != cam.fy || ab->cam.cx != cam.cx ||
-      ab->cam.cy != cam.cy)
-    return fail(c, PLSVO_ERR_INVALID, "raw frames: batch->cam and raw->cam differ in width, height, fx, fy, cx or cy");
+  if (multicam) {
+    if (raw_multicam_check(c, in, ab) != PLSVO_OK) return PLSVO_ERR_INVALID;
+  } else {
+    const plsvo_pinhole_camera& cam = in.cams[0];
+    if (check_pinhole_params(c, cam, "raw-frame camera") != PLSVO_OK) return PLSVO_ERR_INVALID;
+    if (ab->cam.width != W || ab->cam.height != H || ab->cam.fx != cam.fx || ab->cam.fy != cam.fy || ab->cam.cx != cam.cx ||
+        ab->cam.cy != cam.cy)
+      return fail(c, PLSVO_ERR_INVALID, "raw frames: batch->cam and raw->cam differ in width, height, fx, fy, cx or cy");
+  }
   for (int l = 0; l < PLSVO_MAX_LEVELS; ++l)
     if (ab->ref_img[l] || ab->cur_img[l])
       return fail(c, PLSVO_ERR_INVALID, "raw frames: image pointers in the alignment batch (the images come from the raw frames only)");
   const bool chain = (ab->flags & PLSVO_ALIGN_FRAME_CHAIN) != 0;
-  if (!raw->ref_raw || (!chain && !raw->cur_raw)) return fail(c, PLSVO_ERR_INVALID, "raw frames missing (a raw stack is NULL)");
-  if (chain && raw->cur_raw) return fail(c, PLSVO_ERR_INVALID, "raw frames: cur_raw must be NULL with PLSVO_ALIGN_FRAME_CHAIN");
-  if (raw->pitch < (size_t)W) return fail(c, PLSVO_ERR_INVALID, "raw frames: pitch smaller than the image width");
+  if (!in.ref_raw || (!chain && !in.cur_raw)) return fail(c, PLSVO_ERR_INVALID, "raw frames missing (a raw stack is NULL)");
+  if (chain && in.cur_raw) return fail(c, PLSVO_ERR_INVALID, "raw frames: cur_raw must be NULL with PLSVO_ALIGN_FRAME_CHAIN");
+  if (in.pitch < (size_t)W) return fail(c, PLSVO_ERR_INVALID, "raw frames: pitch smaller than the image width");
   if (ap->min_level < 0 || ap->max_level < ap->min_level || ap->n_iter < 1) return fail(c, PLSVO_ERR_INVALID, "level range / n_iter");
   if (ap->max_level > 6) return fail(c, PLSVO_ERR_INVALID, "raw frames: max_level > 6 (one 64x64 level-0 tile holds levels 0..6)");
   if (pb && pb->batch != ab->batch) return fail(c, PLSVO_ERR_INVALID, "alignment and pose-optimiser batches differ in size");
@@ -2102,16 +2243,30 @@ static int raw_run_body(plsvo_ctx* ctx, const plsvo_raw_frames* raw, const plsvo
     if (out && rect->pitch[l] < (size_t)(W >> l)) return fail(c, PLSVO_ERR_INVALID, "rect_out: pitch smaller than the level width");
     top = std::max(top, l);
   }
-  // PinholeCamera's distortion_ flag: without it level 0 is the raw frame itself
-  const bool distortion = fabs(cam.d[0]) > 0.0000001;
-  if (!undistort_pyramid_launch || (distortion && !undistort_map_launch))
+  bool distortion = false;
+  for (int k = 0; k < (multicam ? in.n_cams : 1); ++k) distortion = distortion || distorted(in.cams[k]);
+  if ((multicam ? !undistort_pyramid_multicam_launch : !undistort_pyramid_launch) || (distortion && !undistort_map_launch))
     return fail(c, PLSVO_ERR_CUDA, "raw-frame rectification kernels are not linked into this library", cudaErrorNotSupported);
+  if (multicam && multicam_kernels_present(c, true, pb != nullptr) != PLSVO_OK) return PLSVO_ERR_CUDA;
   // features, poses, outputs and the host-side sizing of the alignment batch (no image is shipped)
   int rc = plsvo_align_upload(ctx, ab);
   if (rc != PLSVO_OK) return rc;
   const size_t B = (size_t)ab->batch;
   if (pb) {
     rc = poseopt_upload_impl(c, pb, pb->T_f_w ? nullptr : c->aa.out_T);
+    if (rc != PLSVO_OK) return rc;
+  }
+  if (multicam) {
+    // pair b is aligned with the undistorted intrinsics of its camera, and its frame's errorMultiplier2 is their |fx|
+    c->h_mc_cams.resize(B);
+    c->h_po_fx.resize(B);
+    for (size_t b = 0; b < B; ++b) {
+      const plsvo_pinhole_camera& k = in.cams[in.cam_of_pair[b]];
+      c->h_mc_cams[b] = plsvo_camera{W, H, 0, 0, k.fx, k.fy, k.cx, k.cy};
+      c->h_po_fx[b] = fabs(k.fx);
+    }
+    rc = multicam_select(c, c->h_mc_cams.data());
+    if (rc == PLSVO_OK && pb) rc = poseopt_fx_select(c, c->h_po_fx.data());
     if (rc != PLSVO_OK) return rc;
   }
   cudaStream_t s = c->stream;
@@ -2140,26 +2295,32 @@ static int raw_run_body(plsvo_ctx* ctx, const plsvo_raw_frames* raw, const plsvo
     c->lvl_uploaded[l] = true;  // present: align_derive_levels derives nothing
   }
   // raw frames: one linear copy per stack when the host layout is uniform (kept on the device), else frame by frame
-  const bool uniform = raw->stride == (size_t)H * raw->pitch;
-  r.src_pitch = uniform ? raw->pitch : (size_t)W;
-  r.src_stride = uniform ? raw->stride : (size_t)H * W;
+  const bool uniform = in.stride == (size_t)H * in.pitch;
+  r.src_pitch = uniform ? in.pitch : (size_t)W;
+  r.src_stride = uniform ? in.stride : (size_t)H * W;
   CK(ensure(c->u_raw, r.src_stride * n_frames));
   uint8_t* d_raw = static_cast<uint8_t*>(c->u_raw.p);
   r.src = d_raw;
-  const uint8_t* stacks[2] = {raw->ref_raw, chain ? nullptr : raw->cur_raw};
+  const uint8_t* stacks[2] = {in.ref_raw, chain ? nullptr : in.cur_raw};
   const size_t per_stack = chain ? B + 1 : B;
   for (int k = 0; k < 2 && stacks[k]; ++k) {
     uint8_t* dst = d_raw + k * per_stack * r.src_stride;
     if (uniform) {
       // the last row of the last frame needs only W of its pitch bytes
-      CK(cudaMemcpyAsync(dst, stacks[k], per_stack * r.src_stride - (raw->pitch - W), cudaMemcpyHostToDevice, s));
+      CK(cudaMemcpyAsync(dst, stacks[k], per_stack * r.src_stride - (in.pitch - W), cudaMemcpyHostToDevice, s));
     } else {
       for (size_t f = 0; f < per_stack; ++f)
-        CK(cudaMemcpy2DAsync(dst + f * r.src_stride, r.src_pitch, stacks[k] + f * raw->stride, raw->pitch, W, H, cudaMemcpyHostToDevice, s));
+        CK(cudaMemcpy2DAsync(dst + f * r.src_stride, r.src_pitch, stacks[k] + f * in.stride, in.pitch, W, H, cudaMemcpyHostToDevice, s));
     }
   }
-  if (distortion) {
-    rc = undistort_map_ensure(c, cam, s);
+  const RawVisit* d_visit = nullptr;
+  if (multicam) {
+    rc = raw_multicam_maps(c, in, (int)B, s);
+    if (rc != PLSVO_OK) return rc;
+    r.map_pitch = map_pitch_of(W);
+    CK(up(c->d_visit, c->h_visit.data(), c->h_visit.size(), s, &d_visit));
+  } else if (distortion) {
+    rc = undistort_map_ensure(c, in.cams[0], s);
     if (rc != PLSVO_OK) return rc;
     r.map_pitch = c->u_map_pitch;
     r.map1 = static_cast<const short2*>(c->u_map1.p), r.map2 = static_cast<const uint16_t*>(c->u_map2.p);
@@ -2170,7 +2331,7 @@ static int raw_run_body(plsvo_ctx* ctx, const plsvo_raw_frames* raw, const plsvo
   rc = align_plan(c, ap, &plan);
   if (rc != PLSVO_OK) return rc;
   CK(kernel_timer(c, 0, s));
-  CK(undistort_pyramid_launch(r, c->num_sms, s));
+  CK(multicam ? undistort_pyramid_multicam_launch(r, d_visit, c->num_sms, s) : undistort_pyramid_launch(r, c->num_sms, s));
   c->launches += 1;
   rc = align_launch_kernel(c, plan, s);
   if (rc == PLSVO_OK && pb) rc = plsvo_poseopt_launch(ctx, pp);
@@ -2196,10 +2357,19 @@ static int raw_run_body(plsvo_ctx* ctx, const plsvo_raw_frames* raw, const plsvo
   return PLSVO_OK;
 }
 
+namespace {
+RawInput raw_input(const plsvo_raw_frames* raw) {
+  return RawInput{false, &raw->cam, 1, nullptr, raw->ref_raw, raw->cur_raw, raw->pitch, raw->stride};
+}
+RawInput raw_input(const plsvo_raw_multicam_frames* raw) {
+  return RawInput{true, raw->cams, raw->n_cams, raw->cam_of_pair, raw->ref_raw, raw->cur_raw, raw->pitch, raw->stride};
+}
+}  // namespace
+
 extern "C" int plsvo_align_raw_batch_run(plsvo_ctx* ctx, const plsvo_raw_frames* raw, const plsvo_align_batch* b,
                                          const plsvo_align_params* p, const plsvo_align_result* o, const plsvo_pyramid_result* rect_out) {
   if (!ctx || !raw || !b || !p || !o) return PLSVO_ERR_INVALID;
-  return settled(CTX(ctx), raw_run_body(ctx, raw, b, p, nullptr, nullptr, o, nullptr, rect_out));
+  return settled(CTX(ctx), raw_run_body(ctx, raw_input(raw), b, p, nullptr, nullptr, o, nullptr, rect_out));
 }
 
 extern "C" int plsvo_track_raw_batch_run(plsvo_ctx* ctx, const plsvo_raw_frames* raw, const plsvo_align_batch* ab,
@@ -2207,7 +2377,22 @@ extern "C" int plsvo_track_raw_batch_run(plsvo_ctx* ctx, const plsvo_raw_frames*
                                          const plsvo_align_result* ao, const plsvo_poseopt_result* po,
                                          const plsvo_pyramid_result* rect_out) {
   if (!ctx || !raw || !ab || !ap || !pb || !pp || !po) return PLSVO_ERR_INVALID;
-  return settled(CTX(ctx), raw_run_body(ctx, raw, ab, ap, pb, pp, ao, po, rect_out));
+  return settled(CTX(ctx), raw_run_body(ctx, raw_input(raw), ab, ap, pb, pp, ao, po, rect_out));
+}
+
+extern "C" int plsvo_align_raw_multicam_batch_run(plsvo_ctx* ctx, const plsvo_raw_multicam_frames* raw, const plsvo_align_batch* b,
+                                                  const plsvo_align_params* p, const plsvo_align_result* o,
+                                                  const plsvo_pyramid_result* rect_out) {
+  if (!ctx || !raw || !b || !p || !o) return PLSVO_ERR_INVALID;
+  return settled(CTX(ctx), raw_run_body(ctx, raw_input(raw), b, p, nullptr, nullptr, o, nullptr, rect_out));
+}
+
+extern "C" int plsvo_track_raw_multicam_batch_run(plsvo_ctx* ctx, const plsvo_raw_multicam_frames* raw, const plsvo_align_batch* ab,
+                                                  const plsvo_align_params* ap, const plsvo_poseopt_batch* pb,
+                                                  const plsvo_poseopt_params* pp, const plsvo_align_result* ao,
+                                                  const plsvo_poseopt_result* po, const plsvo_pyramid_result* rect_out) {
+  if (!ctx || !raw || !ab || !ap || !pb || !pp || !po) return PLSVO_ERR_INVALID;
+  return settled(CTX(ctx), raw_run_body(ctx, raw_input(raw), ab, ap, pb, pp, ao, po, rect_out));
 }
 
 extern "C" int plsvo_match_direct_batch_run(plsvo_ctx* ctx, const plsvo_match_batch* in, const plsvo_match_result* out) {

@@ -229,19 +229,134 @@ __global__ void __launch_bounds__(kRawThreads, kRawCtasPerSm) undistort_pyramid_
   }
 }
 
+// undistort_pyramid_kernel for the frames of several cameras (plsvo_*_raw_multicam_batch_run): the i-th frame of a run
+// is visit[i].frame, rectified with visit[i]'s map, or copied when that is NULL.  The host lists the frames grouped by
+// camera, so that the CTAs resident at one time (dispatched roughly in run order) read the map tiles of only a few
+// cameras and those stay in L2.  The body is undistort_pyramid_kernel's with that choice at the top of the frame loop; it
+// is spelled out again because extracting the shared body into an inlined device function changes the plain kernel's
+// SASS (ptxas reorders its byte-store tail).
+__global__ void __launch_bounds__(kRawThreads, kRawCtasPerSm) undistort_pyramid_multicam_kernel(const RawPyramidArgs a, int frames_per_cta,
+                                                                                               const RawVisit* __restrict__ visit) {
+  __shared__ __align__(16) uint8_t t1[32 * 32];  // level-1 tile
+  __shared__ __align__(16) uint8_t t2[16 * 16];  // level-2 tile, then reused alternately downwards
+  __shared__ __align__(16) uint8_t t3[8 * 8];
+  const int tid = threadIdx.x, tx = tid & 15, ty = tid >> 4;
+  const int x0 = blockIdx.x * kRawTile, y0 = blockIdx.y * kRawTile;
+  const int x = x0 + 4 * tx, y = y0 + 2 * ty;
+  const int W = a.width, H = a.height;
+  const int i0 = blockIdx.z * frames_per_cta, i1 = min(a.B, i0 + frames_per_cta);
+  for (int i = i0; i < i1; ++i) {
+    // the frame and its camera's map: one record, the same for every thread of the CTA
+    const int b = __ldg(&visit[i].frame);
+    const short2* map1 = visit[i].map1;
+    const uint16_t* map2 = visit[i].map2;
+    const uint8_t* src = a.src + (size_t)b * a.src_stride;
+    uint32_t word[2];
+#pragma unroll
+    for (int r = 0; r < 2; ++r) {
+      uint32_t w = 0;
+      if (y + r < H) {
+        if (map1) {
+          const size_t e = (size_t)(y + r) * a.map_pitch + x;
+          const uint4 m1 = __ldg(reinterpret_cast<const uint4*>(map1 + e));
+          const uint2 m2 = __ldg(reinterpret_cast<const uint2*>(map2 + e));
+          w = remap_pixel(src, m1.x, m2.x, W, H, a.src_pitch) | remap_pixel(src, m1.y, m2.x >> 16, W, H, a.src_pitch) << 8 |
+              remap_pixel(src, m1.z, m2.y, W, H, a.src_pitch) << 16 | remap_pixel(src, m1.w, m2.y >> 16, W, H, a.src_pitch) << 24;
+        } else {
+          const uint8_t* row = src + (size_t)(y + r) * a.src_pitch;
+#pragma unroll
+          for (int k = 0; k < 4; ++k)
+            if (x + k < W) w |= (uint32_t)__ldg(row + x + k) << (8 * k);
+        }
+        // pitch is a multiple of 16 and x of 4: the word lies inside the padded row
+        if (a.level[0] && x < (int)a.pitch[0])
+          *reinterpret_cast<uint32_t*>(a.level[0] + (size_t)b * a.stride[0] + (size_t)(y + r) * a.pitch[0] + x) = w;
+      }
+      word[r] = w;
+    }
+    if (a.n_levels < 2) continue;
+    // level 1 from registers: two output bytes per thread
+    const uint32_t o1 = half2x2(word[0], word[1]) & 0xFFFFu;
+    *reinterpret_cast<uint16_t*>(t1 + ty * 32 + 2 * tx) = (uint16_t)o1;
+    if (a.level[1]) {
+      const int ox = x >> 1, oy = y >> 1;  // ox is even and the pitch a multiple of 16: both bytes inside the padded row
+      if (oy < (H >> 1) && ox < (W >> 1))
+        *reinterpret_cast<uint16_t*>(a.level[1] + (size_t)b * a.stride[1] + (size_t)oy * a.pitch[1] + ox) = (uint16_t)o1;
+    }
+    __syncthreads();
+    // levels 2.. from shared memory: thread = (output row, 4-byte output segment), as in pyramid_kernel
+    const uint8_t* in = t1;
+    int in_dim = 32;
+    for (int l = 2; l < a.n_levels; ++l) {
+      const int out_dim = in_dim >> 1;
+      uint8_t* out = (l & 1) ? t3 : t2;
+      const int Wl = W >> l, Hl = H >> l;
+      const int ox0 = x0 >> l, oy0 = y0 >> l;
+      uint8_t* dst = a.level[l] ? a.level[l] + (size_t)b * a.stride[l] : nullptr;
+      if (out_dim >= 4) {
+        const int segs = out_dim >> 2;
+        if (tid < out_dim * segs) {
+          const int oy = tid / segs, sx = (tid - oy * segs) * 4;
+          const uint2 top = *reinterpret_cast<const uint2*>(in + (2 * oy) * in_dim + 2 * sx);
+          const uint2 bot = *reinterpret_cast<const uint2*>(in + (2 * oy + 1) * in_dim + 2 * sx);
+          const uint32_t o = half2x2_word(top.x, top.y, bot.x, bot.y);
+          *reinterpret_cast<uint32_t*>(out + oy * out_dim + sx) = o;
+          const int gx = ox0 + sx, gy = oy0 + oy;
+          if (dst && gy < Hl && gx < Wl) {
+            uint8_t* d = dst + (size_t)gy * a.pitch[l] + gx;
+            if (gx + 4 <= (int)a.pitch[l]) {
+              *reinterpret_cast<uint32_t*>(d) = o;
+            } else {
+              for (int k = 0; k < 4 && gx + k < Wl; ++k) d[k] = (uint8_t)((o >> (8 * k)) & 0xFF);
+            }
+          }
+        }
+      } else {  // 2x2 and 1x1 tiles of the deepest levels: one byte per thread
+        if (tid < out_dim * out_dim) {
+          const int oy = tid / out_dim, ox = tid - oy * out_dim;
+          const uint8_t* p = in + (2 * oy) * in_dim + 2 * ox;
+          const uint8_t v = (uint8_t)(((int)p[0] + (int)p[1] + (int)p[in_dim] + (int)p[in_dim + 1]) / 4);
+          out[tid] = v;
+          if (dst && ox0 + ox < Wl && oy0 + oy < Hl) dst[(size_t)(oy0 + oy) * a.pitch[l] + ox0 + ox] = v;
+        }
+      }
+      __syncthreads();
+      in = out;
+      in_dim = out_dim;
+    }
+  }
+}
+
+
 }  // namespace
 
-cudaError_t undistort_pyramid_launch(const RawPyramidArgs& a, int num_sms, cudaStream_t s) {
+namespace {
+// Frame runs: each CTA loops over a run of frames of one tile.  Enough runs for about eight waves of resident CTAs keep
+// the last wave short.
+dim3 raw_pyramid_grid(const RawPyramidArgs& a, int num_sms, int* per_cta) {
   const int gx = (a.width + kRawTile - 1) / kRawTile, gy = (a.height + kRawTile - 1) / kRawTile;
-  // Frame runs: each CTA loops over a run of frames of one tile.  Enough runs for about eight waves of resident CTAs keep
-  // the last wave short.
   const long long want = (long long)(num_sms > 0 ? num_sms : 1) * kRawCtasPerSm * 8;
   long long runs = (want + gx * gy - 1) / (gx * gy);
   runs = runs < 1 ? 1 : (runs > a.B ? a.B : runs);
   int per = (int)((a.B + runs - 1) / runs);
   per = std::max(per, (a.B + 65534) / 65535);  // gridDim.z <= 65535
   runs = (a.B + per - 1) / per;
-  undistort_pyramid_kernel<<<dim3(gx, gy, (unsigned)runs), kRawThreads, 0, s>>>(a, per);
+  *per_cta = per;
+  return dim3(gx, gy, (unsigned)runs);
+}
+}  // namespace
+
+cudaError_t undistort_pyramid_launch(const RawPyramidArgs& a, int num_sms, cudaStream_t s) {
+  int per = 0;
+  const dim3 grid = raw_pyramid_grid(a, num_sms, &per);
+  undistort_pyramid_kernel<<<grid, kRawThreads, 0, s>>>(a, per);
+  return cudaGetLastError();
+}
+
+cudaError_t undistort_pyramid_multicam_launch(const RawPyramidArgs& a, const RawVisit* visit, int num_sms, cudaStream_t s) {
+  int per = 0;
+  const dim3 grid = raw_pyramid_grid(a, num_sms, &per);
+  undistort_pyramid_multicam_kernel<<<grid, kRawThreads, 0, s>>>(a, per, visit);
   return cudaGetLastError();
 }
 

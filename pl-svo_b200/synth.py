@@ -707,6 +707,28 @@ def make_raw_chain_batch(cam: Camera = EUROC, dist=EUROC_DIST, batch: int = 8, n
     return data, np.ascontiguousarray(raw.cpu().numpy())
 
 
+def make_raw_multicam_batch(cams, dists, cam_of_pair, n_pts: int = 300, n_segs: int = 80, seed: int = 3000,
+                            poseopt: bool = False, scene: Scene | None = None, **align_kw):
+    """make_multicam_batch whose frames are also rendered raw, each pair through its own lens: pair b's reference frame
+    (at T_ref_w) and current frame (at the ground truth T_cur_w_gt) through cams[k] with Brown-Conrady distortion
+    dists[k], k = cam_of_pair[b].  Features, poses and ground truth are those of the undistorted cameras.  Returns
+    (AlignData, (ref_raw, cur_raw) u8 [B,H,W], cameras [B, 4]), or (AlignData, PoseOptData, raw, cameras) when
+    `poseopt`."""
+    scene = scene or Scene()
+    cam_of_pair = np.asarray(cam_of_pair)
+    out = make_multicam_batch(cams, cam_of_pair, n_pts=n_pts, n_segs=n_segs, seed=seed, poseopt=poseopt, scene=scene, **align_kw)
+    al = out[0]
+    B, cam = len(cam_of_pair), cams[0]
+    ref = np.empty((B, cam.height, cam.width), np.uint8)
+    cur = np.empty_like(ref)
+    for k in np.unique(cam_of_pair):
+        idx = np.flatnonzero(cam_of_pair == k)
+        for poses, dst in ((al.T_ref_w, ref), (al.T_cur_w_gt, cur)):
+            pose = torch.tensor(poses[idx], dtype=torch.float64, device=torch.device(align_kw.get("device", "cpu")))
+            dst[idx] = render_distorted(scene, cams[k], dists[k], pose).cpu().numpy()
+    return out[:-1] + ((ref, cur),) + out[-1:]
+
+
 def run_sequence(poses, steps, track_fn):
     """The frame-to-frame chain of FrameHandlerMono::processFrame (src/frame_handler_mono.cpp:263-340) over a sequence:
     new_frame.T_f_w = last_frame.T_f_w (:266), sparse image alignment, pose optimisation, and the result becomes the
