@@ -343,32 +343,37 @@ int plsvo_track_raw_batch_run(plsvo_ctx* ctx, const plsvo_raw_frames* raw, const
 /* ------------------------------------------------------------------------------------------
  * Raw frames from differently calibrated distorted cameras in one batch: the raw-frame calls above with the multicam
  * calls' per-pair intrinsics below.  cams[k] are distorted vk::PinholeCamera arguments (d0..d4 as for
- * plsvo_undistort_batch), all of batch->cam's image size; both frames of pair b are rectified with cams[cam_of_pair[b]],
- * and the pair is then aligned with that camera's fx, fy, cx, cy as its undistorted intrinsics (run_pipeline builds both
- * cameras from the same values).  In the track call frame b's errorMultiplier2 is |fx| of that camera.  Of batch->cam
- * only width and height are used.
+ * plsvo_undistort_batch); both frames of pair b are rectified with cams[cam_of_pair[b]], and the pair is then aligned
+ * with that camera's fx, fy, cx, cy as its undistorted intrinsics (run_pipeline builds both cameras from the same
+ * values).  In the track call frame b's errorMultiplier2 is |fx| of that camera.  Of batch->cam only width and height
+ * are used: they are the slot.
+ * - Slot: every frame of both raw stacks, and of every rect_out level, occupies a slot of batch->cam's size (the raw
+ *   stacks at `pitch` and `stride`).  A camera may be smaller than the slot in either dimension: its frames are its
+ *   width x height in the top-left corner of their slots, at level l (width >> l) x (height >> l).  Raw bytes outside
+ *   that region are never read; cv::remap's constant border applies at the camera's own size.
  * - Pair b's outputs are byte for byte those of plsvo_align_raw_batch_run / plsvo_track_raw_batch_run on that pair with
  *   raw->cam = cams[cam_of_pair[b]], batch->cam carrying its intrinsics, and the same kernel variant.
  * - rect_out as for the raw calls: every non-NULL level, the B reference frames followed by the B current frames, each
- *   rectified with its own camera (plsvo_undistort_batch_run of that frame).  Cameras with fabs(d0) <= 1e-7 copy the frame
- *   and may be mixed with distorted ones.
+ *   rectified with its own camera (plsvo_undistort_batch_run of that frame at the camera's size) in its slot's region,
+ *   the rest of the slot 0.  Cameras with fabs(d0) <= 1e-7 copy the frame and may be mixed with distorted ones.
  * - The maps are built on the device once per camera and kept in a cache of the context separate from the one-camera
  *   cache of plsvo_undistort_batch_run and the raw calls: after a call it holds the maps of exactly the distorted cameras
  *   that call referenced (equal cameras, byte for byte, share one map).  plsvo_last_map_build_ms reports the device time
  *   of the builds the call made, or -1 when it made none.
- * - n_cams < 1, NULL cams or cam_of_pair, an index outside [0, n_cams), a camera whose size differs from batch->cam or
- *   whose parameters plsvo_undistort_batch_run rejects, PLSVO_ALIGN_FRAME_CHAIN (a chained frame belongs to two pairs),
- *   and everything the raw calls reject return PLSVO_ERR_INVALID before anything is queued.  A library built without the
+ * - n_cams < 1, NULL cams or cam_of_pair, an index outside [0, n_cams), a camera wider or taller than batch->cam, or
+ *   below 1 pixel in either dimension, or whose parameters plsvo_undistort_batch_run rejects, a level (aligned or asked
+ *   of rect_out) smaller than one pixel for a camera some pair references, PLSVO_ALIGN_FRAME_CHAIN (a chained frame
+ *   belongs to two pairs), and everything the raw calls reject return PLSVO_ERR_INVALID before anything is queued.  A library built without the
  *   multicam kernels returns PLSVO_ERR_CUDA.  The calls always run upload -> launch -> download and have finished with
  *   the caller's arrays when they return, whatever they return.
- * - Out of scope: per-pair image sizes, ATAN cameras, frame chains, the arrival-gated path.
+ * - Out of scope: a ragged (unpadded) frame layout, ATAN cameras, frame chains, the arrival-gated path.
  * ---------------------------------------------------------------------------------------- */
 typedef struct plsvo_raw_multicam_frames {
   int32_t n_cams, reserved;
-  const plsvo_pinhole_camera* cams; /* [n_cams] distorted cameras (d0..d4 as plsvo_undistort_batch), one image size */
+  const plsvo_pinhole_camera* cams; /* [n_cams] distorted cameras (d0..d4 as plsvo_undistort_batch), each fits the slot */
   const int32_t* cam_of_pair;       /* [B] index into cams: the camera of both frames of pair b */
-  const uint8_t* ref_raw;           /* [B] raw frames */
-  const uint8_t* cur_raw;           /* [B] raw frames */
+  const uint8_t* ref_raw;           /* [B] raw frames, one slot (batch->cam's size) each */
+  const uint8_t* cur_raw;           /* [B] raw frames, one slot (batch->cam's size) each */
   size_t pitch, stride;             /* host layout of both stacks, as plsvo_raw_frames */
 } plsvo_raw_multicam_frames;
 
@@ -417,26 +422,36 @@ int plsvo_track_atan_batch_run(plsvo_ctx* ctx, const plsvo_atan_camera* cam, con
 
 /* ------------------------------------------------------------------------------------------
  * Multicam batches: frame pairs from differently calibrated undistorted pinhole cameras in one call, e.g. a fleet of
- * identical sensors with individual calibrations, or a mix of datasets with the same image size.  These are
- * plsvo_align_batch_run / plsvo_poseopt_batch_run / plsvo_track_batch_run with the intrinsics taken per pair.
+ * identical sensors with individual calibrations, or a mix of datasets and image sizes.  These are
+ * plsvo_align_batch_run / plsvo_poseopt_batch_run / plsvo_track_batch_run with the intrinsics and image size taken per
+ * pair.
+ * - Slot: of batch->cam only width and height are used; they are the slot.  Every pair's frames occupy slots of that
+ *   size in the image stacks, at the batch's pitches and strides.  Pair b's frames are cams[b].width x cams[b].height
+ *   in the top-left corner of their slots, at level l (width >> l) x (height >> l).  cams[b] may be smaller than the
+ *   slot in either dimension; the bytes outside its region (the padding) are never read in a way that reaches a
+ *   result.  Levels derived on the device need no care: the truncating 2x2 mean keeps the region.  In a frame chain
+ *   pairs b and b+1 share a frame, so cams[b] and cams[b+1] must have one size.
  * - Alignment: pair b uses cams[b].fx, fy, cx, cy wherever plsvo_align_batch_run uses batch->cam's: world2cam, cam2world
- *   of bearings not shipped, and the Jacobian factor |fx| / 2^level.  Of batch->cam only width and height are used, and
- *   every cams[b] must have that width and height.  Everything else of `batch` is as for plsvo_align_batch_run: full or
+ *   of bearings not shipped, and the Jacobian factor |fx| / 2^level; and cams[b]'s size wherever it uses the image
+ *   size.  Everything else of `batch` is as for plsvo_align_batch_run: full or
  *   lean bearings, depths, ragged counts and masks, PLSVO_ALIGN_FRAME_CHAIN, NULL levels derived on the device, every
  *   kernel variant (PLSVO_VARIANT).  Pair b's outputs are byte for byte those of plsvo_align_batch_run on the same pair
- *   with batch->cam = cams[b] and the same kernel variant.
+ *   with batch->cam = cams[b] (its frames cut out of the slots) and the same kernel variant.  The slot size enters the
+ *   shared-memory plan, so the variant a call picks may differ from that of the one-camera call: pin it to compare.
  * - Pose optimiser: frame b uses fx[b] (its errorMultiplier2) wherever plsvo_poseopt_batch_run uses batch->fx; the
  *   track call uses |cams[b].fx|, vk::PinholeCamera::errorMultiplier2().  po_batch->fx is ignored by both.
  * - These calls always run upload -> launch -> download on the context's stream, as the ATAN and raw-frame calls do
  *   (not the arrival-gated path), and have finished with the caller's arrays when they return, whatever they return.
- * - NULL cams or fx, a cams[b] whose size differs from batch->cam, a non-finite fx, fy, cx or cy, fx or fy equal to 0,
+ * - NULL cams or fx, a cams[b] wider or taller than batch->cam or below 1 pixel in either dimension, a level (shipped, or
+ *   up to max_level) smaller than one pixel for a cams[b], a frame chain whose size changes between consecutive pairs,
+ *   a non-finite fx, fy, cx or cy, fx or fy equal to 0,
  *   a non-finite or non-positive fx[b], or (track) batch sizes that differ return PLSVO_ERR_INVALID before anything is
  *   queued.  A library built without the multicam kernels returns PLSVO_ERR_CUDA.
  * - The multicam kernels keep the pair's intrinsics in 128 bytes of shared memory per CTA.  A batch whose shared-memory
  *   plan lies within that of the limit is planned for the next kernel variant, as any batch that does not fit; with no
  *   variant left, or PLSVO_VARIANT pinned, it returns PLSVO_ERR_INVALID (DESIGN.md §4.11).
  * - Raw frames: plsvo_*_raw_multicam_batch_run above.
- * - Out of scope: per-pair image sizes, per-pair ATAN cameras, the arrival-gated streamed path, separate upload / launch / download legs, dist.align_sharded, the next-row kernels (direct matching,
+ * - Out of scope: a ragged (unpadded) frame layout, per-pair ATAN cameras, the arrival-gated streamed path, separate upload / launch / download legs, dist.align_sharded, the next-row kernels (direct matching,
  *   seed updates, structure optimisation) and the drop-in shim (one frame per call, nothing to batch).
  * ---------------------------------------------------------------------------------------- */
 int plsvo_align_multicam_batch_run(plsvo_ctx* ctx, const plsvo_camera* cams /* [B] */, const plsvo_align_batch* batch,

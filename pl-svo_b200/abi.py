@@ -180,15 +180,19 @@ class AtanCamera(C.Structure):
                 ("cy", C.c_double), ("d0", C.c_double)]
 
 
-def make_cameras(cameras, cam, batch: int):
-    """plsvo_camera[B] of a multicam call from `cameras`, an array-like [B, 4] of (fx, fy, cx, cy) rows, each with the
-    image size of `cam` (the batch's camera).  Raises ValueError for another shape."""
+def make_cameras(cameras, cam, batch: int, sizes=None):
+    """plsvo_camera[B] of a multicam call from `cameras`, an array-like [B, 4] of (fx, fy, cx, cy) rows.  Each has the
+    image size of `cam` (the batch's camera, whose size is the slot every pair's frames sit in), or with `sizes`, an
+    array-like [B, 2] of (width, height) rows, its own.  Raises ValueError for another shape."""
     k = np.asarray(cameras, dtype=np.float64)
     if k.shape != (batch, 4):
         raise ValueError(f"cameras must have shape [{batch}, 4] (fx, fy, cx, cy per pair), got {list(k.shape)}")
+    wh = np.array([[cam.width, cam.height]] * batch, np.int64).reshape(batch, 2) if sizes is None else np.asarray(sizes)
+    if wh.shape != (batch, 2) or not np.issubdtype(wh.dtype, np.integer):
+        raise ValueError(f"sizes must be integers of shape [{batch}, 2] (width, height per pair), got {wh.dtype} {list(wh.shape)}")
     rec = np.zeros(batch, np.dtype([("size", np.int32, 4), ("k", np.float64, 4)]))
     assert rec.itemsize == C.sizeof(Camera)
-    rec["size"][:, 0], rec["size"][:, 1] = cam.width, cam.height
+    rec["size"][:, :2] = wh
     rec["k"] = k
     return (Camera * batch).from_buffer(rec)  # keeps rec alive
 
@@ -212,10 +216,11 @@ def make_raw_frames(cam: PinholeCamera, raw, batch: int):
     return r, chain, stacks
 
 
-def make_raw_multicam_frames(cams, cam_of_pair, raw, batch: int):
-    """plsvo_raw_multicam_frames for `batch` pairs: cams, a sequence of PinholeCamera structs of one image size;
-    cam_of_pair, the index of every pair's camera; raw, a (ref, cur) pair of u8 [B,H,W] stacks with the same strides
-    (rows may be padded).  Returns (struct, keepalive)."""
+def make_raw_multicam_frames(cams, cam_of_pair, raw, batch: int, slot=None):
+    """plsvo_raw_multicam_frames for `batch` pairs: cams, a sequence of PinholeCamera structs, each no larger than the
+    slot; cam_of_pair, the index of every pair's camera; raw, a (ref, cur) pair of u8 [B,H,W] stacks of the slot's size
+    with the same strides (rows may be padded), frame b in the top-left corner of its slot.  slot: anything with a width
+    and a height (the batch's camera); cams[0]'s size when None.  Returns (struct, keepalive)."""
     if not isinstance(raw, (tuple, list)):
         raise ValueError("raw multicam frames: a (ref, cur) pair of [B,H,W] stacks (frame chains are not supported)")
     if len(cams) < 1:
@@ -224,7 +229,9 @@ def make_raw_multicam_frames(cams, cam_of_pair, raw, batch: int):
     if k.shape != (batch,):
         raise ValueError(f"cam_of_pair must have shape [{batch}], got {list(k.shape)}")
     arr = (PinholeCamera * len(cams))(*cams)
-    r, _, stacks = make_raw_frames(cams[0], raw, batch)
+    frame = PinholeCamera()
+    frame.width, frame.height = (cams[0].width, cams[0].height) if slot is None else (slot.width, slot.height)
+    r, _, stacks = make_raw_frames(frame, raw, batch)
     m = RawMulticamFrames(len(cams), 0, arr, k.ctypes.data_as(C.POINTER(C.c_int32)), r.ref_raw, r.cur_raw, r.pitch, r.stride)
     return m, (arr, k, stacks)
 

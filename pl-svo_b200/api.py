@@ -114,17 +114,20 @@ class SparseImgAlign:
         self.last = out
         return out
 
-    def run(self, data, camera: "ATANCamera | None" = None, cameras=None) -> abi.AlignOut:
+    def run(self, data, camera: "ATANCamera | None" = None, cameras=None, sizes=None) -> abi.AlignOut:
         """run(ref_frames, cur_frames) for a whole batch: returns poses, n_tracked (the reference's
         return value, sparse_img_align.cpp:94), H, killed-segment flags.  camera: an ATANCamera when the frames come from
         one (plsvo_align_atan_batch_run; data.cam then only gives the image size); None for the undistorted pinhole
         data.cam.  cameras: array-like [B, 4] of undistorted pinhole (fx, fy, cx, cy), one row per pair, when the pairs
-        come from differently calibrated cameras of data.cam's image size (plsvo_align_multicam_batch_run)."""
-        _one_camera_model(camera, cameras)
+        come from differently calibrated cameras (plsvo_align_multicam_batch_run).  sizes: with cameras, array-like
+        [B, 2] of every pair's (width, height) when the pairs' frames differ in size: data.cam's size is then the slot
+        each pair's frames sit in, top-left (synth.merge_sizes builds such a batch); data.cam's size for every pair
+        when None."""
+        _one_camera_model(camera, cameras, sizes)
         batch, keep = abi.make_align_batch(data)
         out = abi.AlignOut(data.batch, data.n_segs)
         if cameras is not None:
-            cams = _cameras_arg(cameras, data)
+            cams = _cameras_arg(cameras, data, sizes)
             self.ctx.check(self.ctx.lib.plsvo_align_multicam_batch_run(self.ctx.handle, cams, C.byref(batch),
                                                                        C.byref(self.params), C.byref(out.struct)),
                            "plsvo_align_multicam_batch_run")
@@ -151,12 +154,13 @@ class SparseImgAlign:
         (its images are ignored).  Results are byte-identical to undistortImage followed by the plain host-buffer run().
         rect_levels: levels to bring back as well; returns (AlignOut, {level: [n_frames, H>>l, W>>l]}) then, the frames
         in stack order (the chain, or the reference frames followed by the current ones).
-        cam_of_pair: [B] indices into `camera`, then a sequence of PinholeCamera of data.cam's image size, when the
-        pairs come from differently calibrated lenses (plsvo_align_raw_multicam_batch_run): pair b is rectified with
-        camera[cam_of_pair[b]] and aligned with its fx, fy, cx, cy; data.cam gives only the image size.  raw must then
-        be a (ref, cur) pair of stacks."""
+        cam_of_pair: [B] indices into `camera`, then a sequence of PinholeCamera, when the pairs come from differently
+        calibrated lenses (plsvo_align_raw_multicam_batch_run): pair b is rectified with camera[cam_of_pair[b]] and
+        aligned with its fx, fy, cx, cy.  data.cam gives only the image size of the slot every frame sits in; a camera
+        may be smaller, and its frames then occupy its own size in the top-left corner of their slots (of the raw
+        stacks and of the rect_levels arrays, whose rest is 0).  raw must then be a (ref, cur) pair of stacks."""
         rf, batch, keep = _raw_call_args(camera, raw, data, cam_of_pair)
-        levels, r = _rect_outputs(camera if cam_of_pair is None else camera[0], rf, data.batch, rect_levels)
+        levels, r = _rect_outputs(camera if cam_of_pair is None else data.cam, rf, data.batch, rect_levels)
         out = abi.AlignOut(data.batch, data.n_segs)
         fn, name = ((self.ctx.lib.plsvo_align_raw_batch_run, "plsvo_align_raw_batch_run") if cam_of_pair is None else
                     (self.ctx.lib.plsvo_align_raw_multicam_batch_run, "plsvo_align_raw_multicam_batch_run"))
@@ -199,15 +203,16 @@ class pose_optimizer:
 
 def track(align_data, poseopt_data, max_level: int = 4, min_level: int = 2, n_iter: int = 30, reproj_thresh: float = 2.0,
           po_n_iter: int = 10, po_n_iter_ref: int | None = None, chained: bool = True, ctx: Context | None = None,
-          camera: "ATANCamera | None" = None, cameras=None):
+          camera: "ATANCamera | None" = None, cameras=None, sizes=None):
     """FrameHandlerMono::processFrame's two hot-path calls back to back (src/frame_handler_mono.cpp:272-274, :327-329):
     SparseImgAlign::run on every pair, then pose_optimizer::optimizeGaussNewton on every frame, the pose staying on the
     device in between (chained=True: the pose optimiser starts from the aligned pose of the same batch index).
     camera: an ATANCamera when the frames come from one (plsvo_track_atan_batch_run); poseopt_data.fx is then its
     errorMultiplier2().  cameras: array-like [B, 4] of per-pair undistorted pinhole (fx, fy, cx, cy)
     (plsvo_track_multicam_batch_run); frame b's errorMultiplier2 is then |cameras[b, 0]| and poseopt_data.fx is not used.
+    sizes: with cameras, [B, 2] of every pair's (width, height), as for SparseImgAlign.run.
     Returns (AlignOut, PoseOptOut)."""
-    _one_camera_model(camera, cameras)
+    _one_camera_model(camera, cameras, sizes)
     ctx = ctx or default_context()
     ap = abi.align_params(max_level, min_level, n_iter)
     pp = abi.poseopt_params(reproj_thresh, po_n_iter, -1 if po_n_iter_ref is None else po_n_iter_ref)
@@ -218,7 +223,7 @@ def track(align_data, poseopt_data, max_level: int = 4, min_level: int = 2, n_it
     ao = abi.AlignOut(align_data.batch, align_data.n_segs)
     po = abi.PoseOptOut(poseopt_data.batch, poseopt_data.n_pts, poseopt_data.n_segs)
     if cameras is not None:
-        cams = _cameras_arg(cameras, align_data)
+        cams = _cameras_arg(cameras, align_data, sizes)
         ctx.check(ctx.lib.plsvo_track_multicam_batch_run(ctx.handle, cams, C.byref(ab), C.byref(ap), C.byref(pb), C.byref(pp),
                                                          C.byref(ao.struct), C.byref(po.struct)),
                   "plsvo_track_multicam_batch_run")
@@ -234,19 +239,25 @@ def track(align_data, poseopt_data, max_level: int = 4, min_level: int = 2, n_it
     return ao, po
 
 
-def _one_camera_model(camera, cameras):
+def _one_camera_model(camera, cameras, sizes=None):
     if camera is not None and cameras is not None:
         raise PlsvoError("pass camera= (one ATAN camera) or cameras= (pinhole intrinsics per pair), not both")
+    if sizes is not None and cameras is None:
+        raise PlsvoError("sizes= needs cameras= (the pinhole intrinsics of every pair)")
 
 
-def _cameras_arg(cameras, data):
-    """plsvo_camera[B] for the multicam calls: `cameras` [B, 4] rows (fx, fy, cx, cy), data.cam's image size."""
+def _cameras_arg(cameras, data, sizes=None):
+    """plsvo_camera[B] for the multicam calls: `cameras` [B, 4] rows (fx, fy, cx, cy), and `sizes` [B, 2] rows
+    (width, height) or data.cam's image size."""
     import numpy as np
 
     k = np.asarray(cameras, dtype=np.float64)
     if k.shape != (data.batch, 4):
         raise PlsvoError(f"cameras must have shape [{data.batch}, 4] (fx, fy, cx, cy per pair), got {list(k.shape)}")
-    return abi.make_cameras(k, data.cam, data.batch)
+    try:
+        return abi.make_cameras(k, data.cam, data.batch, sizes)
+    except ValueError as e:
+        raise PlsvoError(str(e)) from None
 
 
 def _frame_fx_arg(fx, batch: int):
@@ -269,7 +280,7 @@ def _raw_call_args(camera, raw, align_data, cam_of_pair=None):
         except (TypeError, AttributeError):
             raise PlsvoError("with cam_of_pair, camera must be a sequence of PinholeCamera") from None
         try:
-            rf, keep_r = abi.make_raw_multicam_frames(structs, cam_of_pair, raw, align_data.batch)
+            rf, keep_r = abi.make_raw_multicam_frames(structs, cam_of_pair, raw, align_data.batch, slot=align_data.cam)
         except ValueError as e:
             raise PlsvoError(str(e)) from None
         chain = False
@@ -312,7 +323,7 @@ def track_raw(camera, raw, align_data, poseopt_data, max_level: int = 4, min_lev
     pb, keep_p = abi.make_poseopt_batch(poseopt_data)
     if chained:
         pb.T_f_w = abi._f64p()
-    levels, r = _rect_outputs(camera if cam_of_pair is None else camera[0], rf, align_data.batch, rect_levels)
+    levels, r = _rect_outputs(camera if cam_of_pair is None else align_data.cam, rf, align_data.batch, rect_levels)
     ao = abi.AlignOut(align_data.batch, align_data.n_segs)
     po = abi.PoseOptOut(poseopt_data.batch, poseopt_data.n_pts, poseopt_data.n_segs)
     fn, name = ((ctx.lib.plsvo_track_raw_batch_run, "plsvo_track_raw_batch_run") if cam_of_pair is None else

@@ -223,15 +223,21 @@ struct PinholePerPair {  // vk::PinholeCamera without distortion, one per pair
   static constexpr bool kAtan = false, kPerPair = true;
 };
 
-// fx, fy, cx, cy of the CTA's current pair (PinholePerPair only): static shared memory, which only the PinholePerPair
-// kernels instantiate.  The 32 bytes cost 128 per CTA (the dynamic region behind them is 128-byte aligned); the host
-// plan reads the compiled size through align_multicam_kernel_static_smem.  Thread 0 fills it from a.cams when the pair
-// starts; every use reads it back, as the pass reads ctl->dscale, so the intrinsics take no registers across the pass.
+// fx, fy, cx, cy of the CTA's current pair (PinholePerPair only), then its frame's width and height as two int32 in
+// K[4]: static shared memory, which only the PinholePerPair kernels instantiate.  The 40 bytes cost 128 per CTA (the
+// dynamic region behind them is 128-byte aligned); the host plan reads the compiled size through
+// align_multicam_kernel_static_smem.  Thread 0 fills it from a.cams when the pair starts; every use reads it back, as the
+// pass reads ctl->dscale, so the intrinsics and the size take no registers across the pass.
 template <class Cam>
 __device__ __forceinline__ double* pair_intrinsics() {
   static_assert(Cam::kPerPair, "only the per-pair camera keeps its intrinsics in shared memory");
-  __shared__ double K[4];
+  __shared__ double K[5];
   return K;
+}
+// The pair's frame size (width, height): the top-left corner of the batch's a.width x a.height slot it sits in.
+template <class Cam>
+__device__ __forceinline__ int* pair_size() {
+  return reinterpret_cast<int*>(pair_intrinsics<Cam>() + 4);
 }
 
 // cam2world: the constructors of PointFeat / LineFeat derive their bearing vectors this way (src/feature.cpp:42,98-99),
@@ -754,6 +760,7 @@ __device__ __forceinline__ void align_pairs(const AlignArgs& a) {
         double* K = pair_intrinsics<Cam>();
         const plsvo_camera& cam = a.cams[b];
         K[0] = cam.fx, K[1] = cam.fy, K[2] = cam.cx, K[3] = cam.cy;
+        pair_size<Cam>()[0] = cam.width, pair_size<Cam>()[1] = cam.height;
       }
     }
     // Host-buffer pipeline with lean inputs: pyramid levels above a.derive_from were not shipped; this CTA forms them
@@ -762,7 +769,10 @@ __device__ __forceinline__ void align_pairs(const AlignArgs& a) {
     // to the persistent grid that is waiting for it.)
     if (a.derive_from >= 0) {
       for (int l = a.derive_from + 1; l <= a.max_level; ++l) {
-        const int cols = a.width >> l, rows = a.height >> l;
+        // the multicam kernels form the pair's own region (its level l depends only on its region at level l-1); the
+        // shared copy of its size is not yet visible here
+        int cols = a.width >> l, rows = a.height >> l;
+        if constexpr (Cam::kPerPair) cols = a.cams[b].width >> l, rows = a.cams[b].height >> l;
         const int pin = (int)a.pitch[l - 1], pout = (int)a.pitch[l];
 #pragma unroll 1
         for (int which = 0; which < 2; ++which) {
@@ -812,7 +822,10 @@ __device__ __forceinline__ void align_pairs(const AlignArgs& a) {
 
     for (int level = a.max_level; level >= a.min_level; --level) {
       PHASE_MARK(kPhPair);
-      const int cols = a.width >> level, rows = a.height >> level;
+      // the pair's frame: the whole slot, or (multicam) its own size in the slot's top-left corner
+      int width = a.width, height = a.height;
+      if constexpr (Cam::kPerPair) width = pair_size<Cam>()[0], height = pair_size<Cam>()[1];
+      const int cols = width >> level, rows = height >> level;
       const int pitch = (int)a.pitch[level];
       const float scale = 1.0f / (float)(1 << level);
       const double dscale = (double)scale;
@@ -823,7 +836,10 @@ __device__ __forceinline__ void align_pairs(const AlignArgs& a) {
       __syncthreads();  // previous level's readers of img_s are done
       if (tid == 0) {
         if (stage) {
-          const uint32_t bytes = (uint32_t)rows * (uint32_t)pitch;
+          uint32_t bytes = (uint32_t)rows * (uint32_t)pitch;
+          // the bulk copy moves whole 16-byte units: the slot's rows * pitch is one, a pair's rows may not be (29 rows of
+          // 40 bytes); rounding up stays inside the slot, whose stride is a multiple of 16 and was planned for
+          if constexpr (Cam::kPerPair) bytes = (bytes + 15u) & ~15u;
           fence_proxy_async();
           mbar_expect_tx(bar, bytes);
           bulk_g2s(img_s, cur_img_g, bytes, bar);
@@ -843,7 +859,7 @@ __device__ __forceinline__ void align_pairs(const AlignArgs& a) {
           const double* epx = a.seg_epx + (so + j) * 2;
           const int sx = (int)(spx[0] * dscale), sy = (int)(spx[1] * dscale);
           const int ex = (int)(epx[0] * dscale), ey = (int)(epx[1] * dscale);
-          if (cam_in_frame(sx, sy, 3, level, a.width, a.height) && cam_in_frame(ex, ey, 3, level, a.width, a.height))
+          if (cam_in_frame(sx, sy, 3, level, width, height) && cam_in_frame(ex, ey, 3, level, width, height))
             N = 1 + ((seg_N0[j] - 1) >> level);
         }
         seg_N[j] = N;

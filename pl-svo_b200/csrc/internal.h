@@ -197,10 +197,14 @@ __attribute__((weak)) cudaError_t undistort_pyramid_launch(const RawPyramidArgs&
 struct RawVisit {           // one frame of a multicam raw batch and the map it is rectified with
   const short2* map1;       // its camera's map ([height][map_pitch], as RawPyramidArgs::map1), or NULL: copy the frame
   const uint16_t* map2;
-  int32_t frame, reserved;  // index into src and every level
+  int32_t frame;            // index into src and every level
+  int32_t width, height;    // its camera's image size: the frame's region in the top-left corner of the slot
+  int32_t map_pitch;        // entries per row of its camera's map
 };
 // The same kernel for frames of several cameras (plsvo_*_raw_multicam_batch_run): visit[0..a.B) lists every frame once,
-// in the order the CTAs' frame runs take them, each with its camera's map (a.map1 / a.map2 are not read).
+// in the order the CTAs' frame runs take them, each with its camera's map and size (a.map1 / a.map2 / a.map_pitch are
+// not read).  a.width x a.height is the slot: every frame's camera fits in it, and a frame's raw image and levels occupy
+// their camera's size in the slot's top-left corner.  The kernel writes nothing of a level outside that region.
 __attribute__((weak)) cudaError_t undistort_pyramid_multicam_launch(const RawPyramidArgs& a, const RawVisit* visit, int num_sms,
                                                                     cudaStream_t s);
 

@@ -1380,19 +1380,38 @@ int plsvo_track_atan_batch_run(plsvo_ctx* ctx, const plsvo_atan_camera* cam, con
 }  // extern "C"
 
 // ------------------------------------------------------------------------------------------------
-// Multicam batches: undistorted pinhole intrinsics per pair, one image size per batch
+// Multicam batches: undistorted pinhole intrinsics and image size per pair, in slots of batch->cam's size
 // ------------------------------------------------------------------------------------------------
 namespace {
 
-// cams[0..B) against the batch: the size of batch->cam, finite intrinsics, fx and fy non-zero.  Nothing is queued here.
-int multicam_check(plsvo_ctx_impl* c, const plsvo_camera* cams, const plsvo_align_batch* b) {
+// A camera of size w x h in a batch whose levels are shipped (or derived up to max_level): every level a one-camera
+// call of that size would touch must be at least one pixel.  A camera of the slot's size is left to the batch's own
+// checks, which the uniform calls have always made.  Returns the first level that is not, or -1.
+int level_under_one_pixel(int w, int h, const plsvo_align_batch* b, int max_level) {
+  const bool chain = (b->flags & PLSVO_ALIGN_FRAME_CHAIN) != 0;
+  for (int l = 0; l < PLSVO_MAX_LEVELS; ++l) {
+    const bool shipped = b->ref_img[l] && (chain || b->cur_img[l]);
+    if ((shipped || l <= max_level) && ((w >> l) <= 0 || (h >> l) <= 0)) return l;
+  }
+  return -1;
+}
+
+// cams[0..B) against the batch: a size that fits the slot (batch->cam's size) and whose levels are at least one pixel,
+// finite intrinsics, fx and fy non-zero; in a frame chain, consecutive pairs share a frame and so a size.  Nothing is
+// queued here.
+int multicam_check(plsvo_ctx_impl* c, const plsvo_camera* cams, const plsvo_align_batch* b, const plsvo_align_params* p) {
   if (!cams) return fail(c, PLSVO_ERR_INVALID, "cams is NULL");
-  char msg[160];
+  char msg[192];
   for (int i = 0; i < b->batch; ++i) {
     const plsvo_camera& k = cams[i];
-    if (k.width != b->cam.width || k.height != b->cam.height) {
-      snprintf(msg, sizeof msg, "cams[%d] is %dx%d, batch->cam is %dx%d: one image size per batch", i, k.width, k.height,
-               b->cam.width, b->cam.height);
+    if (k.width < 1 || k.height < 1 || k.width > b->cam.width || k.height > b->cam.height) {
+      snprintf(msg, sizeof msg, "cams[%d] is %dx%d, batch->cam is %dx%d: every camera must fit inside the batch's image slot", i,
+               k.width, k.height, b->cam.width, b->cam.height);
+      return fail(c, PLSVO_ERR_INVALID, msg);
+    }
+    const int l = k.width == b->cam.width && k.height == b->cam.height ? -1 : level_under_one_pixel(k.width, k.height, b, p->max_level);
+    if (l >= 0) {
+      snprintf(msg, sizeof msg, "cams[%d] is %dx%d: pyramid level %d smaller than one pixel", i, k.width, k.height, l);
       return fail(c, PLSVO_ERR_INVALID, msg);
     }
     if (!std::isfinite(k.fx) || !std::isfinite(k.fy) || !std::isfinite(k.cx) || !std::isfinite(k.cy)) {
@@ -1401,6 +1420,11 @@ int multicam_check(plsvo_ctx_impl* c, const plsvo_camera* cams, const plsvo_alig
     }
     if (k.fx == 0.0 || k.fy == 0.0) {
       snprintf(msg, sizeof msg, "cams[%d].fx and fy must be non-zero", i);
+      return fail(c, PLSVO_ERR_INVALID, msg);
+    }
+    if ((b->flags & PLSVO_ALIGN_FRAME_CHAIN) && i > 0 && (k.width != cams[i - 1].width || k.height != cams[i - 1].height)) {
+      snprintf(msg, sizeof msg, "cams[%d] is %dx%d and cams[%d] is %dx%d: pairs of a frame chain share a frame, so they have one size",
+               i - 1, cams[i - 1].width, cams[i - 1].height, i, k.width, k.height);
       return fail(c, PLSVO_ERR_INVALID, msg);
     }
   }
@@ -1449,7 +1473,7 @@ extern "C" {
 static int align_multicam_body(plsvo_ctx* ctx, const plsvo_camera* cams, const plsvo_align_batch* b,
                                const plsvo_align_params* p, const plsvo_align_result* o) {
   plsvo_ctx_impl* c = CTX(ctx);
-  int rc = multicam_check(c, cams, b);
+  int rc = multicam_check(c, cams, b, p);
   if (rc == PLSVO_OK) rc = multicam_kernels_present(c, true, false);
   if (rc == PLSVO_OK) rc = plsvo_align_upload(ctx, b);
   if (rc == PLSVO_OK) rc = multicam_select(c, cams);
@@ -1486,7 +1510,7 @@ static int track_multicam_body(plsvo_ctx* ctx, const plsvo_camera* cams, const p
                                const plsvo_align_params* ap, const plsvo_poseopt_batch* pb, const plsvo_poseopt_params* pp,
                                const plsvo_align_result* ao, const plsvo_poseopt_result* po) {
   plsvo_ctx_impl* c = CTX(ctx);
-  int rc = multicam_check(c, cams, ab);
+  int rc = multicam_check(c, cams, ab, ap);
   if (rc == PLSVO_OK && pb->batch != ab->batch)
     rc = fail(c, PLSVO_ERR_INVALID, "alignment and pose-optimiser batches differ in size");
   if (rc == PLSVO_OK) rc = multicam_kernels_present(c, true, true);
@@ -2111,9 +2135,9 @@ int raw_multicam_check(plsvo_ctx_impl* c, const RawInput& in, const plsvo_align_
   char msg[160];
   for (int k = 0; k < in.n_cams; ++k) {
     const plsvo_pinhole_camera& cam = in.cams[k];
-    if (cam.width != ab->cam.width || cam.height != ab->cam.height) {
-      snprintf(msg, sizeof msg, "raw multicam frames: cams[%d] is %dx%d, batch->cam is %dx%d: one image size per batch", k, cam.width,
-               cam.height, ab->cam.width, ab->cam.height);
+    if (cam.width < 1 || cam.height < 1 || cam.width > ab->cam.width || cam.height > ab->cam.height) {
+      snprintf(msg, sizeof msg, "raw multicam frames: cams[%d] is %dx%d, batch->cam is %dx%d: every camera must fit inside the batch's image slot",
+               k, cam.width, cam.height, ab->cam.width, ab->cam.height);
       return fail(c, PLSVO_ERR_INVALID, msg);
     }
     snprintf(msg, sizeof msg, "raw multicam frames: cams[%d]", k);
@@ -2133,7 +2157,8 @@ bool distorted(const plsvo_pinhole_camera& cam) { return fabs(cam.d[0]) > 0.0000
 // The maps of a multicam raw call and the order its frames are visited in (c->h_visit).  The cache keeps the maps of
 // the distinct distorted cameras the pairs reference, byte-equal cameras sharing one, and drops the others; a camera
 // already cached is not rebuilt.  Frames [0, B) are the reference frames of the pairs, [B, 2B) the current ones.  The
-// visit order is a counting sort of the frames by map (copied frames last), ascending frame index within a map.
+// visit order is a counting sort of the frames by map (copied frames last), ascending frame index within a map; each
+// record carries its camera's image size and map pitch.
 int raw_multicam_maps(plsvo_ctx_impl* c, const RawInput& in, int B, cudaStream_t s) {
   using CamMap = plsvo_ctx_impl::CamMap;
   std::vector<int> slot_of_cam((size_t)in.n_cams, -2);  // -2: not referenced, -1: no distortion, else its map
@@ -2193,7 +2218,8 @@ int raw_multicam_maps(plsvo_ctx_impl* c, const RawInput& in, int B, cudaStream_t
     RawVisit& v = c->h_visit[start[k]++];
     v.map1 = k < n_maps ? static_cast<const short2*>(c->mc_maps[k]->map1.p) : nullptr;
     v.map2 = k < n_maps ? static_cast<const uint16_t*>(c->mc_maps[k]->map2.p) : nullptr;
-    v.frame = f, v.reserved = 0;
+    const plsvo_pinhole_camera& cam = in.cams[in.cam_of_pair[f < B ? f : f - B]];
+    v.frame = f, v.width = cam.width, v.height = cam.height, v.map_pitch = map_pitch_of(cam.width);
   }
   return PLSVO_OK;
 }
@@ -2231,6 +2257,14 @@ static int raw_run_body(plsvo_ctx* ctx, const RawInput& in, const plsvo_align_ba
   if (ap->min_level < 0 || ap->max_level < ap->min_level || ap->n_iter < 1) return fail(c, PLSVO_ERR_INVALID, "level range / n_iter");
   if (ap->max_level > 6) return fail(c, PLSVO_ERR_INVALID, "raw frames: max_level > 6 (one 64x64 level-0 tile holds levels 0..6)");
   if (pb && pb->batch != ab->batch) return fail(c, PLSVO_ERR_INVALID, "alignment and pose-optimiser batches differ in size");
+  // the smallest width and height of a camera the pairs reference (multicam: each sits in a slot of W x H)
+  int minW = W, minH = H;
+  bool slot_sized = true;
+  for (int b = 0; multicam && b < ab->batch; ++b) {
+    const plsvo_pinhole_camera& k = in.cams[in.cam_of_pair[b]];
+    minW = std::min(minW, k.width), minH = std::min(minH, k.height);
+    slot_sized = slot_sized && k.width == W && k.height == H;
+  }
   // the levels the kernel stores: [min_level, max_level] for alignment, and every level rect_out asks for
   bool want[PLSVO_MAX_LEVELS] = {false};
   int top = ap->max_level;
@@ -2239,7 +2273,8 @@ static int raw_run_body(plsvo_ctx* ctx, const RawInput& in, const plsvo_align_ba
     want[l] = out || (l >= ap->min_level && l <= ap->max_level);
     if (!want[l]) continue;
     if (l > 6) return fail(c, PLSVO_ERR_INVALID, "rect_out: level above 6 (one 64x64 level-0 tile holds levels 0..6)");
-    if ((W >> l) <= 0 || (H >> l) <= 0) return fail(c, PLSVO_ERR_INVALID, "pyramid level smaller than one pixel");
+    if ((W >> l) <= 0 || (H >> l) <= 0 || (minW >> l) <= 0 || (minH >> l) <= 0)
+      return fail(c, PLSVO_ERR_INVALID, "pyramid level smaller than one pixel");
     if (out && rect->pitch[l] < (size_t)(W >> l)) return fail(c, PLSVO_ERR_INVALID, "rect_out: pitch smaller than the level width");
     top = std::max(top, l);
   }
@@ -2257,12 +2292,13 @@ static int raw_run_body(plsvo_ctx* ctx, const RawInput& in, const plsvo_align_ba
     if (rc != PLSVO_OK) return rc;
   }
   if (multicam) {
-    // pair b is aligned with the undistorted intrinsics of its camera, and its frame's errorMultiplier2 is their |fx|
+    // pair b is aligned with the undistorted intrinsics and the image size of its camera, and its frame's
+    // errorMultiplier2 is their |fx|
     c->h_mc_cams.resize(B);
     c->h_po_fx.resize(B);
     for (size_t b = 0; b < B; ++b) {
       const plsvo_pinhole_camera& k = in.cams[in.cam_of_pair[b]];
-      c->h_mc_cams[b] = plsvo_camera{W, H, 0, 0, k.fx, k.fy, k.cx, k.cy};
+      c->h_mc_cams[b] = plsvo_camera{k.width, k.height, 0, 0, k.fx, k.fy, k.cx, k.cy};
       c->h_po_fx[b] = fabs(k.fx);
     }
     rc = multicam_select(c, c->h_mc_cams.data());
@@ -2286,6 +2322,9 @@ static int raw_run_body(plsvo_ctx* ctx, const RawInput& in, const plsvo_align_ba
     total += r.stride[l] * n_frames;
   }
   CK(ensure(c->d_ref_img, total + 256));
+  // frames smaller than the slot: the fused kernel writes only their own region of every level, and the rest of the
+  // slot (read by no result, brought back by rect_out) is cleared here
+  if (!slot_sized) CK(cudaMemsetAsync(c->d_ref_img.p, 0, total, s));
   for (int l = 0; l <= top; ++l) {
     if (!want[l]) continue;
     r.level[l] = static_cast<uint8_t*>(c->d_ref_img.p) + off[l];

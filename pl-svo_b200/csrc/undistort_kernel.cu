@@ -243,11 +243,13 @@ __global__ void __launch_bounds__(kRawThreads, kRawCtasPerSm) undistort_pyramid_
   const int tid = threadIdx.x, tx = tid & 15, ty = tid >> 4;
   const int x0 = blockIdx.x * kRawTile, y0 = blockIdx.y * kRawTile;
   const int x = x0 + 4 * tx, y = y0 + 2 * ty;
-  const int W = a.width, H = a.height;
   const int i0 = blockIdx.z * frames_per_cta, i1 = min(a.B, i0 + frames_per_cta);
   for (int i = i0; i < i1; ++i) {
-    // the frame and its camera's map: one record, the same for every thread of the CTA
+    // the frame, its camera's map and size: one record, the same for every thread of the CTA.  The grid covers the slot
+    // (a.width x a.height); the frame is W x H in its top-left corner.
     const int b = __ldg(&visit[i].frame);
+    const int W = __ldg(&visit[i].width), H = __ldg(&visit[i].height);
+    if (x0 >= W || y0 >= H) continue;  // the tile lies wholly in the slot's padding: nothing of this frame to form
     const short2* map1 = visit[i].map1;
     const uint16_t* map2 = visit[i].map2;
     const uint8_t* src = a.src + (size_t)b * a.src_stride;
@@ -256,8 +258,8 @@ __global__ void __launch_bounds__(kRawThreads, kRawCtasPerSm) undistort_pyramid_
     for (int r = 0; r < 2; ++r) {
       uint32_t w = 0;
       if (y + r < H) {
-        if (map1) {
-          const size_t e = (size_t)(y + r) * a.map_pitch + x;
+        if (map1) {  // x0 < W: the tile's 64 entries lie inside the camera's padded map row (map_pitch, a multiple of 64)
+          const size_t e = (size_t)(y + r) * __ldg(&visit[i].map_pitch) + x;
           const uint4 m1 = __ldg(reinterpret_cast<const uint4*>(map1 + e));
           const uint2 m2 = __ldg(reinterpret_cast<const uint2*>(map2 + e));
           w = remap_pixel(src, m1.x, m2.x, W, H, a.src_pitch) | remap_pixel(src, m1.y, m2.x >> 16, W, H, a.src_pitch) << 8 |
@@ -268,7 +270,9 @@ __global__ void __launch_bounds__(kRawThreads, kRawCtasPerSm) undistort_pyramid_
           for (int k = 0; k < 4; ++k)
             if (x + k < W) w |= (uint32_t)__ldg(row + x + k) << (8 * k);
         }
-        // pitch is a multiple of 16 and x of 4: the word lies inside the padded row
+        // the bytes right of the frame are 0 (the slot's padding stays as the host cleared it); pitch is a multiple of
+        // 16 and x of 4: the word lies inside the padded row
+        if (x + 4 > W) w = x < W ? w & (0xFFFFFFFFu >> (8 * (x + 4 - W))) : 0u;
         if (a.level[0] && x < (int)a.pitch[0])
           *reinterpret_cast<uint32_t*>(a.level[0] + (size_t)b * a.stride[0] + (size_t)(y + r) * a.pitch[0] + x) = w;
       }
@@ -279,9 +283,10 @@ __global__ void __launch_bounds__(kRawThreads, kRawCtasPerSm) undistort_pyramid_
     const uint32_t o1 = half2x2(word[0], word[1]) & 0xFFFFu;
     *reinterpret_cast<uint16_t*>(t1 + ty * 32 + 2 * tx) = (uint16_t)o1;
     if (a.level[1]) {
-      const int ox = x >> 1, oy = y >> 1;  // ox is even and the pitch a multiple of 16: both bytes inside the padded row
-      if (oy < (H >> 1) && ox < (W >> 1))
-        *reinterpret_cast<uint16_t*>(a.level[1] + (size_t)b * a.stride[1] + (size_t)oy * a.pitch[1] + ox) = (uint16_t)o1;
+      const int ox = x >> 1, oy = y >> 1;  // ox is even: both bytes, or the last byte of the frame's row
+      uint8_t* d = a.level[1] + (size_t)b * a.stride[1] + (size_t)oy * a.pitch[1] + ox;
+      if (oy < (H >> 1) && ox + 1 < (W >> 1)) *reinterpret_cast<uint16_t*>(d) = (uint16_t)o1;
+      else if (oy < (H >> 1) && ox < (W >> 1)) *d = (uint8_t)o1;
     }
     __syncthreads();
     // levels 2.. from shared memory: thread = (output row, 4-byte output segment), as in pyramid_kernel
@@ -304,7 +309,7 @@ __global__ void __launch_bounds__(kRawThreads, kRawCtasPerSm) undistort_pyramid_
           const int gx = ox0 + sx, gy = oy0 + oy;
           if (dst && gy < Hl && gx < Wl) {
             uint8_t* d = dst + (size_t)gy * a.pitch[l] + gx;
-            if (gx + 4 <= (int)a.pitch[l]) {
+            if (gx + 4 <= Wl) {
               *reinterpret_cast<uint32_t*>(d) = o;
             } else {
               for (int k = 0; k < 4 && gx + k < Wl; ++k) d[k] = (uint8_t)((o >> (8 * k)) & 0xFF);

@@ -12,7 +12,7 @@ runs on the CPU for tests and on the GPU for the benchmark); nothing is on the p
 from __future__ import annotations
 
 import math
-from dataclasses import dataclass, field
+from dataclasses import dataclass, field, replace
 
 import numpy as np
 import torch
@@ -554,6 +554,45 @@ def take_pairs(data, idx):
         elif isinstance(v, np.ndarray) and v.shape[:1] == (B,):
             setattr(out, f, np.ascontiguousarray(v[idx]))
     return out
+
+
+def merge_sizes(parts, index, slot: Camera | None = None, fill=0, raws=None):
+    """One batch of pairs of several image sizes from one AlignData per size (part k's pairs go to positions index[k],
+    as scatter_batches places them).  Every pair's frames sit in a slot of `slot`'s size (default: the largest width and
+    height of the parts' cameras), the pair's own part.cam.width x height in its top-left corner: the layout of the
+    multicam calls with `sizes=`.  The padding of every level is `fill`, a byte, or a numpy Generator for random bytes.
+    raws: optionally one (ref, cur) pair of raw u8 [B_k, H_k, W_k] stacks per part, merged into slot-sized stacks the
+    same way.  Frame chains are not merged (a chain's pairs share frames, so they have one size).  Returns (AlignData
+    with cam = slot, sizes [B, 2] int32 of (width, height)), plus the merged (ref, cur) raw stacks when `raws` is given.
+    Pose-optimiser batches have no images: scatter_batches merges them."""
+    if any(getattr(p, "frame_pyr", None) is not None for p in parts):
+        raise ValueError("merge_sizes does not take frame chains (frame_pyr)")
+    if slot is None:
+        c0 = parts[0].cam
+        slot = Camera(max(p.cam.width for p in parts), max(p.cam.height for p in parts), c0.fx, c0.fy, c0.cx, c0.cy)
+    if any(p.cam.width > slot.width or p.cam.height > slot.height for p in parts):
+        raise ValueError("every part's camera must fit inside the slot")
+    B = sum(len(i) for i in index)
+
+    def pad(stacks, W, H):
+        shape = (B, H, W)
+        out = fill.integers(0, 256, shape, dtype=np.uint8) if isinstance(fill, np.random.Generator) else np.full(shape, fill, np.uint8)
+        for s, idx in zip(stacks, index):
+            out[np.asarray(idx), : s.shape[1], : s.shape[2]] = s
+        return out
+
+    al = scatter_batches([replace(p, ref_pyr={}, cur_pyr={}) for p in parts], index, B)
+    levels = set.intersection(*(set(p.ref_pyr) for p in parts)) if parts[0].ref_pyr else set()
+    al.ref_pyr = {l: pad([p.ref_pyr[l] for p in parts], slot.width >> l, slot.height >> l) for l in sorted(levels)}
+    al.cur_pyr = {l: pad([p.cur_pyr[l] for p in parts], slot.width >> l, slot.height >> l) for l in sorted(levels)}
+    al.cam = slot
+    sizes = np.zeros((B, 2), np.int32)
+    for p, idx in zip(parts, index):
+        sizes[np.asarray(idx)] = (p.cam.width, p.cam.height)
+    if raws is None:
+        return al, sizes
+    raw = tuple(pad([r[i] for r in raws], slot.width, slot.height) for i in range(2))
+    return al, sizes, raw
 
 
 def multicam_cameras(cams, cam_of_pair) -> np.ndarray:
