@@ -671,6 +671,56 @@ def structopt(abi, data, n_threads: int = 1):
     return out
 
 
+# exit reasons of Point::optimize / LineSeg::optimize in structopt_stats (the same numbers as PO_EXIT_*)
+SO_EXIT_NONE, SO_EXIT_CHI2, SO_EXIT_NAN, SO_EXIT_EPS, SO_EXIT_CAP = range(5)
+SO_CAUSE_CHI2, SO_CAUSE_NAN, SO_CAUSE_EPS = 1, 2, 4
+# the six transposition pairs (tr[0], tr[1]) of a pivoted 3x3 LDLT; bit 2 * tr[0] + tr[1] - 1 of "pivots"
+SO_PIVOTS = ((0, 1), (0, 2), (1, 1), (1, 2), (2, 1), (2, 2))
+
+
+def structopt_stats(abi, data, n_threads: int = 1):
+    """The restated structure optimisation with a record of every point's and every segment end's decisions ->
+    (abi.StructOptOut, pt_stats, seg_stats).  The outputs are those of structopt.  pt_stats is a dict of arrays over the
+    points, seg_stats the same over [n_segs, 2] (the s and e ends):
+      exit, exit_it       SO_EXIT_* and the iteration it was taken at (-1: n_iter = 0); a segment's ends share them
+      cause               bits SO_CAUSE_*: what this end did at the exit (for a segment: which end caused it)
+      pivots              bitmask over the LDLTs factored, bit k for the transposition pair SO_PIVOTS[k]
+      zero                some LDLT took the k == 0 early return (the whole diagonal of A is 0 or NaN)
+      d_zeroed            in an LDLT without the early return, the pseudo-inverse tolerance zeroed a finite D entry
+      d_ratio             smallest min|D| / max|D| over the LDLTs factored
+      A [.., 3, 3], b [.., 3]  the first iteration's normal equations; cond: the 2-norm condition number of that A (inf
+                          when singular, NaN when not finite)"""
+    lib = load(abi)
+    lib.plsvo_oracle_structopt_stats_stride.restype = C.c_int
+    stride = lib.plsvo_oracle_structopt_stats_stride()
+    assert stride == 19
+    fn = lib.plsvo_oracle_structopt_stats
+    fn.restype = C.c_int
+    fn.argtypes = [C.POINTER(abi.StructOptBatch), C.POINTER(abi.StructOptResult), C.POINTER(C.c_double), C.POINTER(C.c_double), C.c_int]
+    b, keep = abi.make_structopt_batch(data)
+    out = abi.StructOptOut(b.n_points, b.n_segs)
+    pst = np.zeros((max(b.n_points, 1), stride))
+    sst = np.zeros((max(b.n_segs, 1), 2, stride))
+    dp = C.POINTER(C.c_double)
+    rc = fn(C.byref(b), C.byref(out.struct), pst.ctypes.data_as(dp), sst.ctypes.data_as(dp), _n_threads(abi, n_threads))
+    if rc != 0:
+        raise RuntimeError(f"oracle structopt_stats failed rc={rc}")
+
+    def unpack(st):
+        A = st[..., 7:16].reshape(st.shape[:-1] + (3, 3)).copy()
+        cond = np.full(st.shape[:-1], np.nan)
+        fin = np.isfinite(A).all((-2, -1))
+        if fin.any():
+            with np.errstate(divide="ignore", invalid="ignore"):
+                s = np.linalg.svd(A[fin], compute_uv=False)
+                cond[fin] = np.where(s[..., -1] > 0, s[..., 0] / s[..., -1], np.inf)
+        return {"exit": st[..., 0].astype(np.int32), "exit_it": st[..., 1].astype(np.int32), "cause": st[..., 2].astype(np.int32),
+                "pivots": st[..., 3].astype(np.int32), "zero": st[..., 4] != 0, "d_zeroed": st[..., 5] != 0,
+                "d_ratio": st[..., 6].copy(), "A": A, "b": st[..., 16:19].copy(), "cond": cond}
+
+    return out, unpack(pst[: b.n_points]), unpack(sst[: b.n_segs])
+
+
 @_recorded
 def ref_structopt(abi, data):
     """Point::optimize / LineSeg::optimize of the reference's own feature3D_impl.cpp -> abi.StructOptOut (iters not observable)."""

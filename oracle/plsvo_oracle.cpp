@@ -1648,9 +1648,11 @@ int plsvo_oracle_match_direct_stats(const plsvo_match_batch* in, const plsvo_mat
 struct Ldlt3 {
   double m[3][3];
   int tr[3];
+  bool zero;  // the k == 0 early return ran: the whole diagonal of A is 0 (or NaN)
 };
 static void ldlt3_compute(const double A[3][3], Ldlt3& f) {
   const int n = 3;
+  f.zero = false;
   for (int i = 0; i < n; ++i)
     for (int j = 0; j < n; ++j) f.m[i][j] = A[i][j];
   for (int k = 0; k < n; ++k) {
@@ -1681,19 +1683,21 @@ static void ldlt3_compute(const double A[3][3], Ldlt3& f) {
     const bool pivot_is_valid = std::fabs(akk) > 0.0;
     if (k == 0 && !pivot_is_valid) {
       for (int j = 0; j < n; ++j) f.tr[j] = j;
+      f.zero = true;
       return;
     }
     if (pivot_is_valid)
       for (int i = k + 1; i < n; ++i) f.m[i][k] /= akk;
   }
 }
+static const double kLdlt3Tol = 1.0 / std::numeric_limits<double>::max();  // the pseudo-inverse's cut of D
 static void ldlt3_solve(const Ldlt3& f, const double b[3], double x[3]) {
   const int n = 3;
   for (int i = 0; i < n; ++i) x[i] = b[i];
   for (int k = 0; k < n; ++k) std::swap(x[k], x[f.tr[k]]);
   for (int i = 0; i < n; ++i)
     for (int j = 0; j < i; ++j) x[i] -= f.m[i][j] * x[j];
-  const double tol = 1.0 / std::numeric_limits<double>::max();
+  const double tol = kLdlt3Tol;
   for (int i = 0; i < n; ++i) {
     if (std::fabs(f.m[i][i]) > tol)
       x[i] /= f.m[i][i];
@@ -1722,83 +1726,180 @@ static void structopt_accumulate(const SE3& T, const double R[3][3], Vec3 pos, V
 }
 static double norm_max3(const double x[3]) { return std::max(std::max(std::fabs(x[0]), std::fabs(x[1])), std::fabs(x[2])); }
 
+// One point's or one segment end's record of plsvo_oracle_structopt_stats (doubles):
+//   exit        why the loop ended: kSoExit* (a segment's two ends share it)
+//   exit_it     the iteration it ended at (-1: n_iter = 0)
+//   cause       what this end did at the exit: 1 chi2 rise (it > 0), 2 NaN step, 4 step within EPS (a segment exits when
+//               either end asks; cause tells which did)
+//   pivots      bitmask over the LDLTs factored: bit 2 * tr[0] + tr[1] - 1 for the transposition pair (tr[0], tr[1])
+//   zero        1 if some LDLT took the k == 0 early return (the whole diagonal 0)
+//   d_zeroed    1 if, in an LDLT without the early return, the pseudo-inverse tolerance zeroed a finite D entry
+//   d_ratio     smallest min|D| / max|D| over the LDLTs factored (NaN sticks; 0 / 0 counts as 0)
+//   A[9], b[3]  the first iteration's normal equations (0: n_iter = 0)
+enum { kSoExitNone = 0, kSoExitChi2 = 1, kSoExitNan = 2, kSoExitEps = 3, kSoExitCap = 4 };
+enum { kSoSExit = 0, kSoSIt = 1, kSoSCause = 2, kSoSPivots = 3, kSoSZero = 4, kSoSZeroed = 5, kSoSRatio = 6, kSoSA = 7, kSoSB = 16,
+       kSoStats = 19 };
+static void structopt_stat_ldlt(double* st, const Ldlt3& f) {
+  if (!st) return;
+  st[kSoSPivots] = (double)((int)st[kSoSPivots] | (1 << (2 * f.tr[0] + f.tr[1] - 1)));
+  if (f.zero) {
+    st[kSoSZero] = 1;
+  } else {
+    for (int i = 0; i < 3; ++i)
+      if (std::fabs(f.m[i][i]) <= kLdlt3Tol) st[kSoSZeroed] = 1;
+  }
+  double lo = std::fabs(f.m[0][0]), hi = lo;
+  for (int i = 1; i < 3; ++i) lo = std::min(lo, std::fabs(f.m[i][i])), hi = std::max(hi, std::fabs(f.m[i][i]));
+  const bool nan = std::isnan(f.m[0][0]) || std::isnan(f.m[1][1]) || std::isnan(f.m[2][2]);
+  keep_min(st[kSoSRatio], nan ? std::numeric_limits<double>::quiet_NaN() : hi > 0 ? lo / hi : 0.0);
+}
+static void structopt_stat_first(double* st, int it, const double A[3][3], const double b[3]) {
+  if (!st || it != 0) return;
+  for (int r = 0; r < 3; ++r) {
+    for (int c = 0; c < 3; ++c) st[kSoSA + 3 * r + c] = A[r][c];
+    st[kSoSB + r] = b[r];
+  }
+}
+static void structopt_stat_init(double* st) {
+  if (!st) return;
+  for (int k = 0; k < kSoStats; ++k) st[k] = 0;
+  st[kSoSExit] = kSoExitNone, st[kSoSIt] = -1, st[kSoSRatio] = std::numeric_limits<double>::infinity();
+}
+static void structopt_stat_exit(double* st, int exit, int it, int cause) {
+  if (st) st[kSoSExit] = exit, st[kSoSIt] = it, st[kSoSCause] = cause;
+}
+
+namespace {
+struct StructOptFrames {
+  std::vector<SE3> T;
+  std::vector<double> R;
+  explicit StructOptFrames(const plsvo_structopt_batch* in) : T(in->n_frames), R((size_t)in->n_frames * 9) {
+    for (int k = 0; k < in->n_frames; ++k) {
+      T[k] = se3_from_pose7(in->T_f_w + 7 * (size_t)k);
+      quat_to_matrix(T[k].q, reinterpret_cast<double(*)[3]>(R.data() + 9 * (size_t)k));
+    }
+  }
+  const double (*Rk(int k) const)[3] { return reinterpret_cast<const double(*)[3]>(R.data() + 9 * (size_t)k); }
+};
+const double kStructOptEps = 0.0000000001;  // plsvo::EPS, global.h:92
+}  // namespace
+
+// Point::optimize of point i; st: its record, or nullptr
+static void structopt_point(const plsvo_structopt_batch* in, const StructOptFrames& F, const plsvo_structopt_result* out, int i, double* st) {
+  structopt_stat_init(st);
+  Vec3 pos{in->pt_pos[3 * (size_t)i], in->pt_pos[3 * (size_t)i + 1], in->pt_pos[3 * (size_t)i + 2]};
+  Vec3 old_point = pos;
+  double chi2 = 0.0;
+  int iters = 0;
+  for (int it = 0; it < in->n_iter_pts; ++it) {
+    double A[3][3] = {{0, 0, 0}, {0, 0, 0}, {0, 0, 0}}, b[3] = {0, 0, 0}, new_chi2 = 0.0;
+    for (int o = in->pt_obs_begin[i]; o < in->pt_obs_begin[i + 1]; ++o) {
+      const int k = in->pt_obs_frame[o];
+      structopt_accumulate(F.T[k], F.Rk(k), pos, Vec3{in->pt_obs_f[3 * (size_t)o], in->pt_obs_f[3 * (size_t)o + 1], in->pt_obs_f[3 * (size_t)o + 2]},
+                           A, b, new_chi2);
+    }
+    structopt_stat_first(st, it, A, b);
+    Ldlt3 f;
+    ldlt3_compute(A, f);
+    structopt_stat_ldlt(st, f);
+    double dp[3];
+    ldlt3_solve(f, b, dp);
+    ++iters;
+    if ((it > 0 && new_chi2 > chi2) || std::isnan(dp[0])) {
+      const bool rise = it > 0 && new_chi2 > chi2;
+      structopt_stat_exit(st, rise ? kSoExitChi2 : kSoExitNan, it, (rise ? 1 : 0) | (std::isnan(dp[0]) ? 2 : 0));
+      pos = old_point;
+      break;
+    }
+    const Vec3 new_point{pos.x + dp[0], pos.y + dp[1], pos.z + dp[2]};
+    old_point = pos;
+    pos = new_point;
+    chi2 = new_chi2;
+    if (norm_max3(dp) <= kStructOptEps) {
+      structopt_stat_exit(st, kSoExitEps, it, 4);
+      break;
+    }
+    if (it + 1 == in->n_iter_pts) structopt_stat_exit(st, kSoExitCap, it, 0);
+  }
+  out->pt_pos[3 * (size_t)i] = pos.x, out->pt_pos[3 * (size_t)i + 1] = pos.y, out->pt_pos[3 * (size_t)i + 2] = pos.z;
+  if (out->pt_iters) out->pt_iters[i] = iters;
+}
+
+// LineSeg::optimize of segment i; st: the records of its s and e ends, or nullptr
+static void structopt_segment(const plsvo_structopt_batch* in, const StructOptFrames& F, const plsvo_structopt_result* out, int i, double* st) {
+  double* ss = st;
+  double* se = st ? st + kSoStats : nullptr;
+  structopt_stat_init(ss);
+  structopt_stat_init(se);
+  const size_t I = (size_t)i;
+  Vec3 sp{in->seg_spos[3 * I], in->seg_spos[3 * I + 1], in->seg_spos[3 * I + 2]};
+  Vec3 ep{in->seg_epos[3 * I], in->seg_epos[3 * I + 1], in->seg_epos[3 * I + 2]};
+  Vec3 old_s = sp, old_e = ep;
+  double chi2s = 0.0, chi2e = 0.0;
+  int iters = 0;
+  for (int it = 0; it < in->n_iter_segs; ++it) {
+    double As[3][3] = {{0, 0, 0}, {0, 0, 0}, {0, 0, 0}}, Ae[3][3] = {{0, 0, 0}, {0, 0, 0}, {0, 0, 0}};
+    double bs[3] = {0, 0, 0}, be[3] = {0, 0, 0}, ns = 0.0, ne = 0.0;
+    for (int o = in->seg_obs_begin[i]; o < in->seg_obs_begin[i + 1]; ++o) {
+      const int k = in->seg_obs_frame[o];
+      const size_t O = (size_t)o;
+      structopt_accumulate(F.T[k], F.Rk(k), sp, Vec3{in->seg_obs_sf[3 * O], in->seg_obs_sf[3 * O + 1], in->seg_obs_sf[3 * O + 2]}, As, bs, ns);
+      structopt_accumulate(F.T[k], F.Rk(k), ep, Vec3{in->seg_obs_ef[3 * O], in->seg_obs_ef[3 * O + 1], in->seg_obs_ef[3 * O + 2]}, Ae, be, ne);
+    }
+    structopt_stat_first(ss, it, As, bs);
+    structopt_stat_first(se, it, Ae, be);
+    Ldlt3 fs, fe;
+    ldlt3_compute(As, fs);
+    ldlt3_compute(Ae, fe);
+    structopt_stat_ldlt(ss, fs);
+    structopt_stat_ldlt(se, fe);
+    double dps[3], dpe[3];
+    ldlt3_solve(fs, bs, dps);
+    ldlt3_solve(fe, be, dpe);
+    ++iters;
+    if ((it > 0 && ns > chi2s) || std::isnan(dps[0]) || (it > 0 && ne > chi2e) || std::isnan(dpe[0])) {
+      const int cs = (it > 0 && ns > chi2s ? 1 : 0) | (std::isnan(dps[0]) ? 2 : 0);
+      const int ce = (it > 0 && ne > chi2e ? 1 : 0) | (std::isnan(dpe[0]) ? 2 : 0);
+      const int exit = ((cs | ce) & 1) ? kSoExitChi2 : kSoExitNan;  // a rise at either end counts as a chi2 exit
+      structopt_stat_exit(ss, exit, it, cs);
+      structopt_stat_exit(se, exit, it, ce);
+      sp = old_s, ep = old_e;
+      break;
+    }
+    const Vec3 new_s{sp.x + dps[0], sp.y + dps[1], sp.z + dps[2]};
+    old_s = sp, sp = new_s, chi2s = ns;
+    const Vec3 new_e{ep.x + dpe[0], ep.y + dpe[1], ep.z + dpe[2]};
+    old_e = ep, ep = new_e, chi2e = ne;
+    if (norm_max3(dps) <= kStructOptEps || norm_max3(dpe) <= kStructOptEps) {
+      structopt_stat_exit(ss, kSoExitEps, it, norm_max3(dps) <= kStructOptEps ? 4 : 0);
+      structopt_stat_exit(se, kSoExitEps, it, norm_max3(dpe) <= kStructOptEps ? 4 : 0);
+      break;
+    }
+    if (it + 1 == in->n_iter_segs) structopt_stat_exit(ss, kSoExitCap, it, 0), structopt_stat_exit(se, kSoExitCap, it, 0);
+  }
+  out->seg_spos[3 * I] = sp.x, out->seg_spos[3 * I + 1] = sp.y, out->seg_spos[3 * I + 2] = sp.z;
+  out->seg_epos[3 * I] = ep.x, out->seg_epos[3 * I + 1] = ep.y, out->seg_epos[3 * I + 2] = ep.z;
+  if (out->seg_iters) out->seg_iters[i] = iters;
+}
+
 int plsvo_oracle_structopt_batch(const plsvo_structopt_batch* in, const plsvo_structopt_result* out, int n_threads) {
   if (!in || !out) return PLSVO_ERR_INVALID;
-  std::vector<SE3> T(in->n_frames);
-  std::vector<double> R((size_t)in->n_frames * 9);
-  for (int k = 0; k < in->n_frames; ++k) {
-    T[k] = se3_from_pose7(in->T_f_w + 7 * (size_t)k);
-    quat_to_matrix(T[k].q, reinterpret_cast<double(*)[3]>(R.data() + 9 * (size_t)k));
-  }
-  auto Rk = [&](int k) { return reinterpret_cast<const double(*)[3]>(R.data() + 9 * (size_t)k); };
-  const double kEps = 0.0000000001;  // plsvo::EPS, global.h:92
-  parallel_for(in->n_points, n_threads, [&](int i) {
-    Vec3 pos{in->pt_pos[3 * (size_t)i], in->pt_pos[3 * (size_t)i + 1], in->pt_pos[3 * (size_t)i + 2]};
-    Vec3 old_point = pos;
-    double chi2 = 0.0;
-    int iters = 0;
-    for (int it = 0; it < in->n_iter_pts; ++it) {
-      double A[3][3] = {{0, 0, 0}, {0, 0, 0}, {0, 0, 0}}, b[3] = {0, 0, 0}, new_chi2 = 0.0;
-      for (int o = in->pt_obs_begin[i]; o < in->pt_obs_begin[i + 1]; ++o) {
-        const int k = in->pt_obs_frame[o];
-        structopt_accumulate(T[k], Rk(k), pos, Vec3{in->pt_obs_f[3 * (size_t)o], in->pt_obs_f[3 * (size_t)o + 1], in->pt_obs_f[3 * (size_t)o + 2]},
-                             A, b, new_chi2);
-      }
-      Ldlt3 f;
-      ldlt3_compute(A, f);
-      double dp[3];
-      ldlt3_solve(f, b, dp);
-      ++iters;
-      if ((it > 0 && new_chi2 > chi2) || std::isnan(dp[0])) {
-        pos = old_point;
-        break;
-      }
-      const Vec3 new_point{pos.x + dp[0], pos.y + dp[1], pos.z + dp[2]};
-      old_point = pos;
-      pos = new_point;
-      chi2 = new_chi2;
-      if (norm_max3(dp) <= kEps) break;
-    }
-    out->pt_pos[3 * (size_t)i] = pos.x, out->pt_pos[3 * (size_t)i + 1] = pos.y, out->pt_pos[3 * (size_t)i + 2] = pos.z;
-    if (out->pt_iters) out->pt_iters[i] = iters;
-  });
-  parallel_for(in->n_segs, n_threads, [&](int i) {
-    const size_t I = (size_t)i;
-    Vec3 sp{in->seg_spos[3 * I], in->seg_spos[3 * I + 1], in->seg_spos[3 * I + 2]};
-    Vec3 ep{in->seg_epos[3 * I], in->seg_epos[3 * I + 1], in->seg_epos[3 * I + 2]};
-    Vec3 old_s = sp, old_e = ep;
-    double chi2s = 0.0, chi2e = 0.0;
-    int iters = 0;
-    for (int it = 0; it < in->n_iter_segs; ++it) {
-      double As[3][3] = {{0, 0, 0}, {0, 0, 0}, {0, 0, 0}}, Ae[3][3] = {{0, 0, 0}, {0, 0, 0}, {0, 0, 0}};
-      double bs[3] = {0, 0, 0}, be[3] = {0, 0, 0}, ns = 0.0, ne = 0.0;
-      for (int o = in->seg_obs_begin[i]; o < in->seg_obs_begin[i + 1]; ++o) {
-        const int k = in->seg_obs_frame[o];
-        const size_t O = (size_t)o;
-        structopt_accumulate(T[k], Rk(k), sp, Vec3{in->seg_obs_sf[3 * O], in->seg_obs_sf[3 * O + 1], in->seg_obs_sf[3 * O + 2]}, As, bs, ns);
-        structopt_accumulate(T[k], Rk(k), ep, Vec3{in->seg_obs_ef[3 * O], in->seg_obs_ef[3 * O + 1], in->seg_obs_ef[3 * O + 2]}, Ae, be, ne);
-      }
-      Ldlt3 fs, fe;
-      ldlt3_compute(As, fs);
-      ldlt3_compute(Ae, fe);
-      double dps[3], dpe[3];
-      ldlt3_solve(fs, bs, dps);
-      ldlt3_solve(fe, be, dpe);
-      ++iters;
-      if ((it > 0 && ns > chi2s) || std::isnan(dps[0]) || (it > 0 && ne > chi2e) || std::isnan(dpe[0])) {
-        sp = old_s, ep = old_e;
-        break;
-      }
-      const Vec3 new_s{sp.x + dps[0], sp.y + dps[1], sp.z + dps[2]};
-      old_s = sp, sp = new_s, chi2s = ns;
-      const Vec3 new_e{ep.x + dpe[0], ep.y + dpe[1], ep.z + dpe[2]};
-      old_e = ep, ep = new_e, chi2e = ne;
-      if (norm_max3(dps) <= kEps || norm_max3(dpe) <= kEps) break;
-    }
-    out->seg_spos[3 * I] = sp.x, out->seg_spos[3 * I + 1] = sp.y, out->seg_spos[3 * I + 2] = sp.z;
-    out->seg_epos[3 * I] = ep.x, out->seg_epos[3 * I + 1] = ep.y, out->seg_epos[3 * I + 2] = ep.z;
-    if (out->seg_iters) out->seg_iters[i] = iters;
-  });
+  const StructOptFrames F(in);
+  parallel_for(in->n_points, n_threads, [&](int i) { structopt_point(in, F, out, i, nullptr); });
+  parallel_for(in->n_segs, n_threads, [&](int i) { structopt_segment(in, F, out, i, nullptr); });
+  return PLSVO_OK;
+}
+
+// The same optimisation, also recording every feature's decisions (test infrastructure: which pivots, exits and degenerate
+// systems a test batch reaches): pt_stats [n_points][stride], seg_stats [n_segs][2 (s, e)][stride] doubles, laid out as
+// described above structopt_stat_ldlt.
+int plsvo_oracle_structopt_stats_stride(void) { return kSoStats; }
+int plsvo_oracle_structopt_stats(const plsvo_structopt_batch* in, const plsvo_structopt_result* out, double* pt_stats, double* seg_stats,
+                                 int n_threads) {
+  if (!in || !out || (in->n_points > 0 && !pt_stats) || (in->n_segs > 0 && !seg_stats)) return PLSVO_ERR_INVALID;
+  const StructOptFrames F(in);
+  parallel_for(in->n_points, n_threads, [&](int i) { structopt_point(in, F, out, i, pt_stats + (size_t)kSoStats * i); });
+  parallel_for(in->n_segs, n_threads, [&](int i) { structopt_segment(in, F, out, i, seg_stats + (size_t)2 * kSoStats * i); });
   return PLSVO_OK;
 }
 

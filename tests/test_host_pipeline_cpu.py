@@ -100,7 +100,7 @@ def test_fast_gpu_tier_files_against_the_host_model_with_oracle_backed_kernels(h
     root = os.path.dirname(HERE)
     env = dict(os.environ, PLSVO_LIB=hostmodel, PLSVO_FAKE_CUDA="lazy", PLSVO_FAKE_ORACLE=os.path.join(root, "oracle", "libplsvo_oracle.so"))
     files = [os.path.join(HERE, f) for f in ("test_gpu_golden.py", "test_gpu_poseopt.py", "test_pyramid.py", "test_align2d.py", "test_matcher.py",
-                                             "test_structopt.py", "test_depth_filter.py")]
+                                             "test_structopt.py", "test_gpu_structopt_cases.py", "test_depth_filter.py")]
     p = subprocess.run([sys.executable, "-m", "pytest", *files, "-q", "-m", "gpu", "-p", "no:cacheprovider", "-k",
                         "not shim_optimize_structure_on_the_gpu"],  # that case links the CUDA library directly
                        env=env, capture_output=True, text=True, timeout=1200)

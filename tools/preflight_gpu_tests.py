@@ -25,7 +25,7 @@ import sys
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 DEFAULT_FILES = ["test_gpu_abi_errors.py", "test_gpu_golden.py", "test_gpu_poseopt.py", "test_gpu_poseopt_cases.py", "test_gpu_track.py", "test_gpu_align.py",
                  "test_gpu_align_variants.py", "test_pyramid.py", "test_gpu_pyramid_cases.py",
-                 "test_align2d.py", "test_matcher.py", "test_gpu_direct_match_cases.py", "test_structopt.py", "test_depth_filter.py", "test_gpu_seed_schedules.py", "test_zz_gpu_chain.py", "test_zz_gpu_word_pitch.py"]
+                 "test_align2d.py", "test_matcher.py", "test_gpu_direct_match_cases.py", "test_structopt.py", "test_gpu_structopt_cases.py", "test_depth_filter.py", "test_gpu_seed_schedules.py", "test_zz_gpu_chain.py", "test_zz_gpu_word_pitch.py"]
 NEEDS_REAL_KERNELS = "not depths_instead and not bearings_derived and not shim_optimize_structure_on_the_gpu"
 
 
