@@ -227,9 +227,8 @@ void atan_bearing(const vk::ATANCamera& cam, const double* px, double* f) {
 }
 
 // as align_one of plsvo_oracle.cpp; NULL bearings are formed with the camera's cam2world
-void atan_align_one(const plsvo_atan_camera* C, const plsvo_align_batch* B, const plsvo_align_params* P,
+void atan_align_one(const vk::ATANCamera& cam, const plsvo_align_batch* B, const plsvo_align_params* P,
                     const plsvo_align_result* out, int b) {
-  const vk::ATANCamera cam(C->width, C->height, C->fx, C->fy, C->cx, C->cy, C->d0);
   // the pinhole fields the included precompute reads (errorMultiplier2, image size) hold the ATAN camera's
   plsvo_align_batch Bd = *B;
   Bd.cam.fx = cam.fx_, Bd.cam.fy = cam.fy_, Bd.cam.cx = cam.cx_, Bd.cam.cy = cam.cy_;
@@ -307,7 +306,22 @@ int plsvo_oracle_atan_align_batch(const plsvo_atan_camera* cam, const plsvo_alig
   if (params->max_level < params->min_level || params->min_level < 0 || params->max_level >= PLSVO_MAX_LEVELS)
     return PLSVO_ERR_INVALID;
   if (cam->width != batch->cam.width || cam->height != batch->cam.height) return PLSVO_ERR_INVALID;
-  parallel_for(batch->batch, n_threads, [&](int b) { atan_align_one(cam, batch, params, out, b); });
+  const vk::ATANCamera c(cam->width, cam->height, cam->fx, cam->fy, cam->cx, cam->cy, cam->d0);
+  parallel_for(batch->batch, n_threads, [&](int b) { atan_align_one(c, batch, params, out, b); });
+  return PLSVO_OK;
+}
+
+// The same, with the camera given by its derived members fx_, fy_, cx_, cy_ (pixels) and d0, as the device kernels
+// receive it (AlignArgs): the host model of the tests answers the ATAN kernels with this, so that no normalisation
+// round trip W * (fx_ / W) can move a member by an ulp.  batch->cam supplies the image size.
+int plsvo_oracle_atan_align_batch_members(double fx_, double fy_, double cx_, double cy_, double d0, const plsvo_align_batch* batch,
+                                          const plsvo_align_params* params, const plsvo_align_result* out, int n_threads) {
+  if (!batch || !params || !out) return PLSVO_ERR_INVALID;
+  if (params->max_level < params->min_level || params->min_level < 0 || params->max_level >= PLSVO_MAX_LEVELS)
+    return PLSVO_ERR_INVALID;
+  vk::ATANCamera c(batch->cam.width, batch->cam.height, 1.0, 1.0, 0.5, 0.5, d0);
+  c.fx_ = fx_, c.fy_ = fy_, c.cx_ = cx_, c.cy_ = cy_;
+  parallel_for(batch->batch, n_threads, [&](int b) { atan_align_one(c, batch, params, out, b); });
   return PLSVO_OK;
 }
 

@@ -51,6 +51,8 @@ def load(abi):
     P = C.POINTER
     lib.plsvo_oracle_atan_align_batch.restype = C.c_int
     lib.plsvo_oracle_atan_align_batch.argtypes = [P(abi.AtanCamera), P(abi.AlignBatch), P(abi.AlignParams), P(abi.AlignResult), C.c_int]
+    lib.plsvo_oracle_atan_align_batch_members.restype = C.c_int
+    lib.plsvo_oracle_atan_align_batch_members.argtypes = [C.c_double] * 5 + [P(abi.AlignBatch), P(abi.AlignParams), P(abi.AlignResult), C.c_int]
     for name in ("plsvo_oracle_atan_cam2world", "plsvo_oracle_atan_world2cam"):
         fn = getattr(lib, name)
         fn.restype = None
@@ -68,6 +70,19 @@ def align(abi, camera, data, params=None, n_threads: int = 1):
     batch, keep = abi.make_align_batch(data)
     out = abi.AlignOut(data.batch, data.n_segs)
     rc = lib.plsvo_oracle_atan_align_batch(C.byref(camera.struct), C.byref(batch), C.byref(params), C.byref(out.struct), n_threads)
+    if rc != 0:
+        raise RuntimeError(f"ATAN oracle align failed rc={rc}")
+    return out
+
+
+def align_members(abi, camera, data, params=None, n_threads: int = 1):
+    """align() with the camera given by its derived members fx_, fy_, cx_, cy_ and d0 (the device kernels' AlignArgs)."""
+    lib = load(abi)
+    params = params or abi.align_params(data.max_level, data.min_level)
+    batch, keep = abi.make_align_batch(data)
+    out = abi.AlignOut(data.batch, data.n_segs)
+    rc = lib.plsvo_oracle_atan_align_batch_members(camera.fx_, camera.fy_, camera.cx_, camera.cy_, camera.s_, C.byref(batch), C.byref(params),
+                                                   C.byref(out.struct), n_threads)
     if rc != 0:
         raise RuntimeError(f"ATAN oracle align failed rc={rc}")
     return out

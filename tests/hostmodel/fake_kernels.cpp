@@ -11,6 +11,7 @@
 //               Levels that the real kernel derives itself (AlignArgs::derive_from) are derived here the same way; the
 //               arrival gate is honoured pair by pair, advancing the other streams only as far as the gate requires.
 //   pyramid   : the real computation (truncating 2x2 mean), it is the producer of derived levels.
+//               The ATAN kernels (align_atan_kernel_*) are the same model: the camera model changes no byte they read.
 //   pose-opt  : out_num_pt[b] = digest of frame b's inputs; out_T[b] = T_f_w[b].
 //   the next-row kernels exist in the oracle-backed mode only (below); otherwise they report cudaErrorNotSupported.
 //
@@ -20,7 +21,9 @@
 // device-layout arguments to the CPU oracle instead of digesting them, so that the GPU tier's own test files can be run
 // here against the unchanged host code (a pre-flight of those files and of the host paths they take, never a parity
 // statement: oracle is compared with oracle).  Inputs the oracle cannot take (depth-only features, bearings not shipped)
-// are refused with cudaErrorNotSupported.
+// are refused with cudaErrorNotSupported.  The ATAN kernels are answered by the oracle's ATAN path
+// (plsvo_oracle_atan_align_batch_members, oracle/atan_oracle.cpp), looked up in the same library or, when that is the plain
+// oracle, in libplsvo_atan_oracle.so next to it; it forms NULL bearings itself, as the ATAN kernels do.
 #include <dlfcn.h>
 #include <string.h>
 
@@ -168,6 +171,9 @@ struct OracleApi {
   int (*structopt)(const plsvo_structopt_batch*, const plsvo_structopt_result*, int) = nullptr;
   int (*seed)(const plsvo_seed_batch*, const plsvo_seed_result*, int) = nullptr;
   int (*line_seed)(const plsvo_line_seed_batch*, const plsvo_line_seed_result*, int) = nullptr;
+  // optional: the ATAN alignment, camera given by its members fx_, fy_, cx_, cy_ and d0
+  int (*atan_align)(double, double, double, double, double, const plsvo_align_batch*, const plsvo_align_params*,
+                    const plsvo_align_result*, int) = nullptr;
 };
 
 const OracleApi* oracle() {
@@ -187,6 +193,14 @@ const OracleApi* oracle() {
         api.structopt = reinterpret_cast<decltype(api.structopt)>(dlsym(h, "plsvo_oracle_structopt_batch"));
         api.seed = reinterpret_cast<decltype(api.seed)>(dlsym(h, "plsvo_oracle_seed_update_batch"));
         api.line_seed = reinterpret_cast<decltype(api.line_seed)>(dlsym(h, "plsvo_oracle_line_seed_update_batch"));
+        const char* atan_sym = "plsvo_oracle_atan_align_batch_members";
+        api.atan_align = reinterpret_cast<decltype(api.atan_align)>(dlsym(h, atan_sym));
+        if (!api.atan_align) {
+          std::string sib(path);
+          sib = sib.substr(0, sib.find_last_of('/') + 1) + "libplsvo_atan_oracle.so";
+          if (void* ha = dlopen(sib.c_str(), RTLD_NOW | RTLD_LOCAL))
+            api.atan_align = reinterpret_cast<decltype(api.atan_align)>(dlsym(ha, atan_sym));
+        }
       }
       if (api.align && api.poseopt && api.align2d && api.align1d && api.match && api.structopt && api.seed && api.line_seed) state = 1;
       else fakecuda::error(std::string("PLSVO_FAKE_ORACLE: cannot load the oracle from ") + path);
@@ -197,7 +211,7 @@ const OracleApi* oracle() {
 
 int host_threads() { return (int)std::max(1u, std::thread::hardware_concurrency()); }
 
-void align_by_oracle(const OracleApi* o, const plsvo::AlignArgs& a) {
+void align_by_oracle(const OracleApi* o, const plsvo::AlignArgs& a, bool atan) {
   plsvo_align_batch b;
   memset(&b, 0, sizeof b);
   b.batch = a.B, b.n_pts = a.n_pts, b.n_segs = a.n_segs;
@@ -224,7 +238,7 @@ void align_by_oracle(const OracleApi* o, const plsvo::AlignArgs& a) {
   memset(a.out_iters, 0, B * 4 * PLSVO_MAX_LEVELS), memset(a.out_status, 0, B * 4);
   memset(a.out_patch_iters, 0, B * 4), memset(a.out_patch_levels, 0, B * 4);
   if (a.n_segs > 0) memset(a.out_seg_killed, 0, B * (size_t)a.n_segs);
-  const int rc = o->align(&b, &p, &r, host_threads(), 0);
+  const int rc = atan ? o->atan_align(a.fx, a.fy, a.cx, a.cy, a.atan_s, &b, &p, &r, host_threads()) : o->align(&b, &p, &r, host_threads(), 0);
   if (rc != PLSVO_OK) fakecuda::error("the oracle refused the alignment batch the host code built");
 }
 
@@ -283,13 +297,20 @@ cudaError_t weight_selftest_launch(uint32_t, uint32_t, unsigned long long* d_mis
   });
 }
 
-cudaError_t align_kernel_launch(const AlignArgs& a, int grid, int threads, int min_blocks, size_t smem_bytes, cudaStream_t s) {
+// the pinhole and the ATAN kernels (atan: AlignArgs::fx..cy hold the members fx_..cy_, atan_s is d0)
+static cudaError_t launch_align(const AlignArgs& a, int grid, int threads, int min_blocks, size_t smem_bytes, cudaStream_t s, bool atan) {
   if (grid < 1 || threads < 32 || min_blocks < 1 || smem_bytes > 232448) {
     fakecuda::error("align_kernel_launch: launch configuration out of range");
     return cudaErrorInvalidConfiguration;
   }
   const OracleApi* orc = oracle();
-  if (orc && ((a.n_pts > 0 && (!a.pt_f || !a.pt_pos)) || (a.n_segs > 0 && (!a.seg_sf || !a.seg_ef || !a.seg_spos || !a.seg_epos)))) {
+  if (orc && atan && !orc->atan_align) {
+    fakecuda::error("oracle-backed model kernel: the oracle library has no ATAN path (build oracle/libplsvo_atan_oracle.so)");
+    return cudaErrorNotSupported;
+  }
+  // the ATAN oracle forms NULL bearings with the camera's cam2world, as the ATAN kernels do; the pinhole oracle cannot
+  const bool no_bearings = !atan && ((a.n_pts > 0 && !a.pt_f) || (a.n_segs > 0 && (!a.seg_sf || !a.seg_ef)));
+  if (orc && (no_bearings || (a.n_pts > 0 && !a.pt_pos) || (a.n_segs > 0 && (!a.seg_spos || !a.seg_epos)))) {
     // depth-only features / bearings not shipped are outside the oracle's inputs: refused, unless the caller asked for the
     // digest kernel on such batches (the bench pre-flight, whose end-to-end legs ship lean inputs)
     if (!getenv("PLSVO_FAKE_LEAN_DIGEST")) {
@@ -300,7 +321,7 @@ cudaError_t align_kernel_launch(const AlignArgs& a, int grid, int threads, int m
   }
   auto run = std::make_shared<AlignRun>();
   run->a = a, run->stream = s;
-  return fakecuda::enqueue(s, [run, orc]() {
+  return fakecuda::enqueue(s, [run, orc, atan]() {
     const AlignArgs& a = run->a;
     if (run->next == 0) {
       if (!fakecuda::check(a.work_counter, 4, "work counter")) return true;
@@ -319,9 +340,21 @@ cudaError_t align_kernel_launch(const AlignArgs& a, int grid, int threads, int m
       run->next = b + 1;
       *a.work_counter = (unsigned)run->next;
     }
-    if (orc) align_by_oracle(orc, a);
+    if (orc) align_by_oracle(orc, a, atan);
     return true;
   });
+}
+
+cudaError_t align_kernel_launch(const AlignArgs& a, int grid, int threads, int min_blocks, size_t smem_bytes, cudaStream_t s) {
+  return launch_align(a, grid, threads, min_blocks, smem_bytes, s, false);
+}
+
+cudaError_t align_atan_kernel_prepare(int threads, int min_blocks, size_t smem_bytes, int* ctas_per_sm) {
+  return align_kernel_prepare(threads, min_blocks, smem_bytes, ctas_per_sm);
+}
+
+cudaError_t align_atan_kernel_launch(const AlignArgs& a, int grid, int threads, int min_blocks, size_t smem_bytes, cudaStream_t s) {
+  return launch_align(a, grid, threads, min_blocks, smem_bytes, s, true);
 }
 
 size_t poseopt_smem_bytes(int n_pts, int n_segs) { return 4096 + 24 * ((size_t)n_pts + (size_t)n_segs); }

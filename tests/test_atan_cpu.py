@@ -109,3 +109,123 @@ def test_oracle_atan_path_equals_the_reference_bit_for_bit(pkg, abi, synth, orac
         for f in ("T_cur_w", "n_tracked", "H", "seg_killed", "iters", "status"):
             np.testing.assert_array_equal(getattr(got, f), getattr(ref, f), err_msg=f)
         assert got.n_tracked.min() > 0
+
+
+# ------------------------------------------------------------------------------------------------
+# the model in extended precision at the d0 values and cut-offs of tests/test_gpu_atan_cases.py
+# ------------------------------------------------------------------------------------------------
+
+EDGE_D0 = [-0.3, 1e-9, 0.93, 1.4, 2.4]
+EPS = np.finfo(np.float64).eps
+
+
+def _ld_cam2world(cam, px):
+    """cam2world in np.longdouble from the camera's double members; also returns r_d and whether the factor applies."""
+    L = np.longdouble
+    px = np.asarray(px, L)
+    x, y = (px[:, 0] - L(cam.cx_)) / L(cam.fx_), (px[:, 1] - L(cam.cy_)) / L(cam.fy_)
+    rd = np.sqrt(x * x + y * y)
+    r = np.tan(rd * L(cam.s_)) * L(cam.tans_inv_) if cam.s_ != 0.0 else rd
+    applies = rd > L(0.01)
+    factor = np.where(applies, r / np.where(applies, rd, 1), L(1))
+    x, y = factor * x, factor * y
+    n = np.sqrt(x * x + y * y + 1)
+    return np.stack([x / n, y / n, 1 / n], -1), rd, applies
+
+
+def _ld_world2cam(cam, xyz):
+    L = np.longdouble
+    xyz = np.asarray(xyz, L)
+    u, v = xyz[:, 0] / xyz[:, 2], xyz[:, 1] / xyz[:, 2]
+    r = np.sqrt(u * u + v * v)
+    applies = ~((r < L(0.001)) | (cam.s_ == 0.0))
+    f = L(cam.s_inv_) * np.arctan(r * L(cam.tans_)) / np.where(r > 0, r, 1)
+    factor = np.where(applies, f, L(1))
+    return np.stack([L(cam.cx_) + L(cam.fx_) * factor * u, L(cam.cy_) + L(cam.fy_) * factor * v], -1), applies
+
+
+@pytest.mark.parametrize("d0", EDGE_D0)
+def test_camera_model_against_extended_precision(pkg, abi, synth, oracle_atan, d0):
+    """api.ATANCamera and the C++ stand-in against the model evaluated in long double: the same branch at both cut-offs
+    (at r_d == 0.01 exactly and at r == 0 too) and within a few ulp, scaled by the conditioning of tan near pi/2."""
+    import test_gpu_atan_cases as cases
+
+    for cam in (vga_atan(pkg, synth, d0), cases._telephoto(pkg, synth, cases.C2W_FX, d0)[0]):
+        _model_against_extended_precision(abi, oracle_atan, cases, cam, d0)
+
+
+def _model_against_extended_precision(abi, oracle_atan, cases, cam, d0):
+    rng = np.random.default_rng(12)
+    c = np.array([cam.cx_, cam.cy_])
+    px = np.concatenate([np.stack([rng.uniform(0, 640, 3000), rng.uniform(0, 480, 3000)], -1),
+                         [c, cases.rd_exactly_001(cam) if cam.fx_ == cases.C2W_FX else c],  # the VGA camera has no such pixel
+                         c + cases._in_annulus(rng, (200,), 0.0, 0.0099 * cam.fx_, (0, 0)),     # inside r_d <= 0.01
+                         c + cases._in_annulus(rng, (200,), 0.0101 * cam.fx_, 0.011 * cam.fx_, (0, 0))])  # just outside
+    ld, rd, applies = _ld_cam2world(cam, px)
+    assert rd[3000] == 0 and cases.rd_of(cam, px[3001:3002])[0] == (0.01 if cam.fx_ == cases.C2W_FX else 0) and not applies[3000:3202].any() and applies[3202:].all()
+    x = np.abs(rd * abs(d0)).astype(np.float64)
+    kappa = np.where(x > 0, x * (1 + np.tan(x) ** 2) / np.maximum(np.abs(np.tan(x)), 1e-300), 1.0)  # relative condition of tan
+    keep = np.abs(x - np.pi / 2) > 1e-3  # at the pole itself no precision is defined
+    tol = 8 * EPS * (1 + kappa[keep, None])
+    for got in (cam.cam2world(px), oracle_atan.cam2world(abi, cam, px)):
+        assert (np.abs(got[keep] - ld[keep].astype(np.float64)) <= tol).all()
+        # the branch: with the other one the bearing would be off by the factor's jump, far beyond the tolerance
+        flat = px[~applies]
+        xy = (flat - c) / [cam.fx_, cam.fy_]
+        n = np.sqrt((xy ** 2).sum(1) + 1)
+        np.testing.assert_array_equal(got[~applies], np.concatenate([xy / n[:, None], 1 / n[:, None]], 1))
+
+    xyz = np.concatenate([rng.uniform(-1, 1, (3000, 2)), rng.uniform(0.5, 3, (3000, 1))], -1)
+    ring = lambda r0, r1, n: np.concatenate([cases._in_annulus(rng, (n,), r0, r1, (0, 0)), np.ones((n, 1))], 1)
+    xyz = np.concatenate([xyz, [[0, 0, 1], [0, 0, 2.5]], ring(0, 0.00099, 200), ring(0.00101, 0.0011, 200)])
+    ld, applies = _ld_world2cam(cam, xyz)
+    assert not applies[3000:3202].any() and applies[3202:].all() == (d0 != 0)
+    for got in (cam.world2cam(xyz), oracle_atan.world2cam(abi, cam, xyz)):
+        np.testing.assert_allclose(got, ld.astype(np.float64), rtol=8 * EPS, atol=8 * EPS * 640)
+        np.testing.assert_array_equal(got[3000:3002], [c, c])  # r = 0: the guard, not 0/0
+
+
+def test_atan_cases_fixtures_reach_their_branches(pkg, abi, synth, oracle_atan):
+    """The fixtures of tests/test_gpu_atan_cases.py, built here as there: every cut-off fixture is inside (or just
+    outside) its cut-off, r_d == 0.01 is hit exactly, d0 = 2.4 has feature pixels past pi/2, the non-square camera is told
+    apart from its transpose by the oracle, and the world2cam pairs compared on the GPU stay inside r < 0.001."""
+    import test_gpu_atan_cases as cases
+    from test_gpu_align import ROT_TOL, TRANS_TOL
+
+    cam, data = cases.cam2world_disc_batch(pkg, synth, "cpu")
+    rd = cases.rd_of(cam, cases.feature_px(data))
+    assert rd.max() == 0.01 and (rd == 0.01).sum() == data.batch and (rd == 0).sum() == data.batch
+    cam, ring = cases.cam2world_disc_batch(pkg, synth, "cpu", ring=True)
+    rd = cases.rd_of(cam, cases.feature_px(ring))
+    assert rd.min() > 0.01 and rd.max() <= 0.011
+
+    cam, data = cases.world2cam_disc_batch(pkg, synth, "cpu")
+    flat = cases._telephoto(pkg, synth, cases.W2C_FX, 0.0)[0]
+    r0 = cases.projected_r(data, data.T_cur_w)
+    assert r0.max() < 0.0005 and r0[0, 0] == 0.0
+    data = through(cam, data)
+    inside, ref = cases.world2cam_inside_pairs(abi, oracle_atan, cam, flat, data)
+    assert inside[0] and inside.sum() >= data.batch // 2, inside
+    assert cases.projected_r(data, ref.T_cur_w)[inside].max() < 0.001
+
+    cam, data = cases.d0_edge_batch(pkg, synth, "cpu", 2.4)
+    assert (cases.rd_of(cam, cases.feature_px(data)) * 2.4 > np.pi / 2).sum() > 0
+
+    cam, swapped = cases.nonsquare_cameras(pkg)
+    assert (cam.fx_, cam.fy_) == (swapped.fy_, swapped.fx_) or abs(cam.fx_ - swapped.fy_) < 1e-12
+    data = cases.nonsquare_batch(pkg, synth, "cpu")
+    a, b = oracle_atan.align(abi, cam, data, n_threads=8), oracle_atan.align(abi, swapped, data, n_threads=8)
+    ang, rel = synth.pose_error(a.T_cur_w, b.T_cur_w)
+    assert ((ang > 100 * ROT_TOL) | (rel > 100 * TRANS_TOL)).all(), (ang.min(), rel.min())
+    # the host model's entry takes the members the kernels receive: the same bytes as the normalised camera's
+    m = oracle_atan.align_members(abi, cam, data, n_threads=8)
+    for f in ("T_cur_w", "n_tracked", "H", "seg_killed", "iters", "status", "patch_iters", "patch_levels"):
+        np.testing.assert_array_equal(getattr(m, f), getattr(a, f), err_msg=f)
+
+
+def through(cam, data):
+    """Full bearings of api.ATANCamera.cam2world, as test_gpu_atan.through(lean=False)."""
+    d = copy.copy(data)
+    d.pt_f = np.ascontiguousarray(cam.cam2world(data.pt_px))
+    d.seg_sf, d.seg_ef = (np.ascontiguousarray(cam.cam2world(x)) for x in (data.seg_spx, data.seg_epx))
+    return d

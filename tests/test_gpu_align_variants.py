@@ -26,9 +26,10 @@ def _num_sms():
     return torch.cuda.get_device_properties(0).multi_processor_count if torch.cuda.is_available() else 132
 
 
-def _long_segments(synth, data, rng, n_long):
+def _long_segments(synth, data, rng, n_long, atan=None):
     """Stretch the segments across a 720p image: about half of them nearly horizontal over more than 1024 px (more than
-    64 samples at level 0: three trips of a warp), the rest anywhere (mostly two trips)."""
+    64 samples at level 0: three trips of a warp), the rest anywhere (mostly two trips).  atan: the ATAN camera the
+    frames were rendered through; the endpoints are then lifted through its rays."""
     import torch
 
     B, S = data.seg_spx.shape[:2]
@@ -42,7 +43,10 @@ def _long_segments(synth, data, rng, n_long):
 
     def lift(px):
         p = torch.tensor(px)
-        d = torch.stack([(p[..., 0] - data.cam.cx) / data.cam.fx, (p[..., 1] - data.cam.cy) / data.cam.fy, torch.ones_like(p[..., 0])], -1)
+        if atan is not None:
+            d = synth.atan_rays(atan, p[..., 0], p[..., 1])
+        else:
+            d = torch.stack([(p[..., 0] - data.cam.cx) / data.cam.fx, (p[..., 1] - data.cam.cy) / data.cam.fy, torch.ones_like(p[..., 0])], -1)
         return (d / d.norm(dim=-1, keepdim=True)).numpy(), scene.intersect(R, t, d).numpy()
 
     data.seg_spx, data.seg_epx = np.ascontiguousarray(spx), np.ascontiguousarray(epx)
@@ -52,18 +56,24 @@ def _long_segments(synth, data, rng, n_long):
     return data
 
 
-def _make(name, synth, dev):
-    """(data, max_level, min_level) of one case."""
+def _make(name, synth, dev, atan=None):
+    """(data, max_level, min_level) of one case.  atan(cam): the ATAN camera of an image size, through which the frames
+    are rendered and the features lifted (None: the pinhole camera)."""
+    mk = synth.make_align_batch
+    if atan is not None:
+        def mk(cam=synth.VGA, **kw):
+            return synth.make_align_batch(cam=cam, atan=atan(cam), **kw)
+
     if name == "vga":  # the bench shape
-        return synth.make_align_batch(batch=16, n_pts=300, n_segs=80, device=dev, seed=6000), 4, 2
+        return mk(batch=16, n_pts=300, n_segs=80, device=dev, seed=6000), 4, 2
     if name == "boundaries":
         n = len(BOUNDARY_COUNTS)
-        d = synth.make_align_batch(batch=n, n_pts=300, n_segs=80, device=dev, seed=6100)
+        d = mk(batch=n, n_pts=300, n_segs=80, device=dev, seed=6100)
         d.pt_count = np.array(BOUNDARY_COUNTS, np.int32)
         d.seg_count = np.array([[0, 1, 13, 31, 33, 80][i % 6] for i in range(n)], np.int32)
         return d, 4, 2
     if name == "edge":  # as test_align_edge_cases: masks, ragged counts, empty / points-only / segments-only pairs, border
-        d = synth.make_align_batch(batch=12, n_pts=96, n_segs=40, device=dev, seed=3400, margin=2)
+        d = mk(batch=12, n_pts=96, n_segs=40, device=dev, seed=3400, margin=2)
         rng = np.random.default_rng(5)
         d.pt_valid = (rng.uniform(size=(12, 96)) > 0.2).astype(np.uint8)
         d.seg_valid = (rng.uniform(size=(12, 40)) > 0.2).astype(np.uint8)
@@ -74,24 +84,24 @@ def _make(name, synth, dev):
         d.seg_count[7] = 0
         return d, 4, 2
     if name == "long_segments":
-        d = synth.make_align_batch(cam=synth.HD720, batch=4, n_pts=200, n_segs=12, max_level=2, min_level=0,
-                                   device=dev, seed=6200, motion_t=0.004, motion_r=0.0012, margin=24)
-        return _long_segments(synth, d, np.random.default_rng(6201), 6), 2, 0
+        d = mk(cam=synth.HD720, batch=4, n_pts=200, n_segs=12, max_level=2, min_level=0,
+               device=dev, seed=6200, motion_t=0.004, motion_r=0.0012, margin=24)
+        return _long_segments(synth, d, np.random.default_rng(6201), 6, atan and atan(synth.HD720)), 2, 0
     if name == "720p":  # the finest level is not staged in shared memory
-        return synth.make_align_batch(cam=synth.HD720, batch=6, n_pts=500, n_segs=150, device=dev, seed=6300), 4, 2
+        return mk(cam=synth.HD720, batch=6, n_pts=500, n_segs=150, device=dev, seed=6300), 4, 2
     if name in ("levels_5_3", "levels_2_0"):
         max_level, min_level = (5, 3) if name == "levels_5_3" else (2, 0)
         s = 1 << (4 - min(4, max_level))
-        d = synth.make_align_batch(batch=6, n_pts=128, n_segs=32, max_level=max_level, min_level=min_level, device=dev,
-                                   seed=6400 + max_level, motion_t=0.03 / s, motion_r=0.01 / s)
+        d = mk(batch=6, n_pts=128, n_segs=32, max_level=max_level, min_level=min_level, device=dev,
+               seed=6400 + max_level, motion_t=0.03 / s, motion_r=0.01 / s)
         return d, max_level, min_level
     if name == "zero_motion":  # identical images: a segment's zero mean residual makes the step NaN, stop_ on every pair
-        d = synth.make_align_batch(cam=synth.QVGA, batch=4, n_pts=40, n_segs=8, max_level=3, min_level=1, seed=21, margin=32,
-                                   motion_t=0.0, motion_r=0.0, device=dev)
+        d = mk(cam=synth.QVGA, batch=4, n_pts=40, n_segs=8, max_level=3, min_level=1, seed=21, margin=32,
+               motion_t=0.0, motion_r=0.0, device=dev)
         return d, 3, 1
     if name == "ragged_pairs_per_cta":  # about three pairs of different sizes per persistent CTA, one CTA per SM
         B = 3 * _num_sms()
-        d = synth.make_align_batch(batch=B, n_pts=72, n_segs=14, device=dev, seed=6500)
+        d = mk(batch=B, n_pts=72, n_segs=14, device=dev, seed=6500)
         rng = np.random.default_rng(6501)
         d.pt_count = rng.integers(0, 73, B).astype(np.int32)
         d.seg_count = rng.integers(0, 15, B).astype(np.int32)
@@ -101,7 +111,7 @@ def _make(name, synth, dev):
         return d, 4, 2
     if name.startswith("pts_"):  # thousands of points per pair
         n_pts = int(name[4:])
-        return synth.make_align_batch(batch=3, n_pts=n_pts, n_segs=80, device=dev, seed=6600 + n_pts), 4, 2
+        return mk(batch=3, n_pts=n_pts, n_segs=80, device=dev, seed=6600 + n_pts), 4, 2
     raise KeyError(name)
 
 

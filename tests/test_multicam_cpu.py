@@ -68,8 +68,8 @@ print("RESULT", rcs, rc_uniform, msg)
 
 
 def test_well_formed_calls_reach_the_kernel_check(hostmodel, tmp_path):
-    """Well-formed multicam calls pass validation and report the missing kernels (PLSVO_ERR_CUDA), as the ATAN calls do
-    in a library built without theirs."""
+    """Well-formed multicam calls pass validation and report the missing kernels (PLSVO_ERR_CUDA), as any call does in
+    a library built without its kernels."""
     script = tmp_path / "well_formed.py"
     script.write_text(_WELL_FORMED)
     root = os.path.dirname(HERE)
