@@ -451,7 +451,8 @@ int plsvo_track_atan_batch_run(plsvo_ctx* ctx, const plsvo_atan_camera* cam, con
  *   plan lies within that of the limit is planned for the next kernel variant, as any batch that does not fit; with no
  *   variant left, or PLSVO_VARIANT pinned, it returns PLSVO_ERR_INVALID (DESIGN.md §4.11).
  * - Raw frames: plsvo_*_raw_multicam_batch_run above.
- * - Out of scope: a ragged (unpadded) frame layout, per-pair ATAN cameras, the arrival-gated streamed path, separate upload / launch / download legs, dist.align_sharded, the next-row kernels (direct matching,
+ * - ATAN (FOV) cameras per pair: plsvo_*_atan_multicam_batch_run below.
+ * - Out of scope: a ragged (unpadded) frame layout, pinhole and ATAN pairs in one batch, the arrival-gated streamed path, separate upload / launch / download legs, dist.align_sharded, the next-row kernels (direct matching,
  *   seed updates, structure optimisation) and the drop-in shim (one frame per call, nothing to batch).
  * ---------------------------------------------------------------------------------------- */
 int plsvo_align_multicam_batch_run(plsvo_ctx* ctx, const plsvo_camera* cams /* [B] */, const plsvo_align_batch* batch,
@@ -463,6 +464,38 @@ int plsvo_track_multicam_batch_run(plsvo_ctx* ctx, const plsvo_camera* cams /* [
                                    const plsvo_align_params* al_params, const plsvo_poseopt_batch* po_batch,
                                    const plsvo_poseopt_params* po_params, const plsvo_align_result* al_out,
                                    const plsvo_poseopt_result* po_out);
+
+/* ------------------------------------------------------------------------------------------
+ * Multicam ATAN batches: frame pairs from differently calibrated ATAN (FOV) cameras in one call, e.g. a fleet of FOV-lens
+ * sensors with individual fx, fy, cx, cy and d0, of one size or several.  These are plsvo_align_atan_batch_run /
+ * plsvo_track_atan_batch_run with the camera taken per pair, in the slot layout of the multicam calls above.
+ * - Slot: of batch->cam only width and height are used; they are the slot.  Pair b's frames are
+ *   cams[b].width x cams[b].height in the top-left corner of their slots, as for plsvo_align_multicam_batch_run.
+ * - Alignment: pair b uses cams[b]'s members fx_, fy_, cx_, cy_, s_, s_inv_, tans_, tans_inv_ (derived from its constructor
+ *   arguments exactly as plsvo_align_atan_batch_run derives them) wherever that call uses the batch's camera.  Everything
+ *   else of `batch` is as for plsvo_align_atan_batch_run: full or lean bearings, depths, ragged counts and masks,
+ *   PLSVO_ALIGN_FRAME_CHAIN (frames of one size), NULL levels derived on the device, every kernel variant.  Pair b's
+ *   outputs are byte for byte those of plsvo_align_atan_batch_run on the same pair with cams[b] at its own size (its
+ *   frames cut out of the slots) and the same kernel variant.
+ * - Track: frame b's errorMultiplier2 is fx_ = cams[b].width * cams[b].fx; po_batch->fx is ignored.
+ * - These calls always run upload -> launch -> download on the context's stream (not the arrival-gated path) and have
+ *   finished with the caller's arrays when they return, whatever they return.
+ * - NULL cams; a cams[b] wider or taller than the slot, below one pixel, or with a level (shipped, or up to max_level)
+ *   smaller than one pixel; a frame chain whose size changes between consecutive pairs; a non-finite parameter, fx <= 0
+ *   or fy <= 0, or a derived focal length out of range for any cams[b] (the index is in the message); or (track) batch
+ *   sizes that differ return PLSVO_ERR_INVALID before anything is queued.  A library built without the ATAN multicam
+ *   kernels returns PLSVO_ERR_CUDA.
+ * - The kernels keep the pair's members, size and distortion terms in 128 bytes of shared memory per CTA, planned for as
+ *   for the multicam kernels (DESIGN.md §4.14).
+ * - Out of scope: pinhole and ATAN pairs in one batch, raw frames, the arrival-gated path, a ragged layout, the next-row
+ *   kernels and the drop-in shim.
+ * ---------------------------------------------------------------------------------------- */
+int plsvo_align_atan_multicam_batch_run(plsvo_ctx* ctx, const plsvo_atan_camera* cams /* [B] */, const plsvo_align_batch* batch,
+                                        const plsvo_align_params* params, const plsvo_align_result* out);
+int plsvo_track_atan_multicam_batch_run(plsvo_ctx* ctx, const plsvo_atan_camera* cams /* [B] */, const plsvo_align_batch* al_batch,
+                                        const plsvo_align_params* al_params, const plsvo_poseopt_batch* po_batch,
+                                        const plsvo_poseopt_params* po_params, const plsvo_align_result* al_out,
+                                        const plsvo_poseopt_result* po_out);
 
 /* ------------------------------------------------------------------------------------------
  * Feature alignment (SURVEY.md §8f "next", rank 1): feature_alignment::align2D,

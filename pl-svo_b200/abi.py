@@ -197,6 +197,19 @@ def make_cameras(cameras, cam, batch: int, sizes=None):
     return (Camera * batch).from_buffer(rec)  # keeps rec alive
 
 
+def make_atan_cameras(cams, cam_of_pair, batch: int):
+    """plsvo_atan_camera[B] of an ATAN multicam call: entry b is cams[cam_of_pair[b]], cams a sequence of AtanCamera
+    structs.  Raises ValueError for an empty `cams`, or a cam_of_pair of another shape or with an index out of range."""
+    if len(cams) < 1:
+        raise ValueError("ATAN multicam call: at least one camera")
+    k = np.asarray(cam_of_pair)
+    if k.shape != (batch,) or not np.issubdtype(k.dtype, np.integer):
+        raise ValueError(f"cam_of_pair must be integers of shape [{batch}], got {k.dtype} {list(k.shape)}")
+    if batch and (k.min() < 0 or k.max() >= len(cams)):
+        raise ValueError(f"cam_of_pair indexes {len(cams)} cameras, got values in [{k.min()}, {k.max()}]")
+    return (AtanCamera * batch)(*(cams[int(i)] for i in k))
+
+
 def make_raw_frames(cam: PinholeCamera, raw, batch: int):
     """plsvo_raw_frames for `batch` pairs from raw u8 frames: one array [B+1,H,W] (a frame chain) or a pair (ref, cur) of
     [B,H,W] arrays with the same strides.  Rows may be padded.  Returns (struct, chain, keepalive)."""
@@ -525,6 +538,10 @@ ABI_SYMBOLS = [
     ("plsvo_align_atan_batch_run", C.c_int, [C.c_void_p, _P(AtanCamera), _P(AlignBatch), _P(AlignParams), _P(AlignResult)]),
     ("plsvo_track_atan_batch_run", C.c_int, [C.c_void_p, _P(AtanCamera), _P(AlignBatch), _P(AlignParams), _P(PoseOptBatch),
                                              _P(PoseOptParams), _P(AlignResult), _P(PoseOptResult)]),
+    ("plsvo_align_atan_multicam_batch_run", C.c_int, [C.c_void_p, _P(AtanCamera), _P(AlignBatch), _P(AlignParams),
+                                                      _P(AlignResult)]),
+    ("plsvo_track_atan_multicam_batch_run", C.c_int, [C.c_void_p, _P(AtanCamera), _P(AlignBatch), _P(AlignParams),
+                                                      _P(PoseOptBatch), _P(PoseOptParams), _P(AlignResult), _P(PoseOptResult)]),
     ("plsvo_align_multicam_batch_run", C.c_int, [C.c_void_p, _P(Camera), _P(AlignBatch), _P(AlignParams), _P(AlignResult)]),
     ("plsvo_poseopt_multicam_batch_run", C.c_int, [C.c_void_p, _f64p, _P(PoseOptBatch), _P(PoseOptParams), _P(PoseOptResult)]),
     ("plsvo_track_multicam_batch_run", C.c_int, [C.c_void_p, _P(Camera), _P(AlignBatch), _P(AlignParams), _P(PoseOptBatch),

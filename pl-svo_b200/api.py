@@ -114,7 +114,7 @@ class SparseImgAlign:
         self.last = out
         return out
 
-    def run(self, data, camera: "ATANCamera | None" = None, cameras=None, sizes=None) -> abi.AlignOut:
+    def run(self, data, camera: "ATANCamera | None" = None, cameras=None, sizes=None, cam_of_pair=None) -> abi.AlignOut:
         """run(ref_frames, cur_frames) for a whole batch: returns poses, n_tracked (the reference's
         return value, sparse_img_align.cpp:94), H, killed-segment flags.  camera: an ATANCamera when the frames come from
         one (plsvo_align_atan_batch_run; data.cam then only gives the image size); None for the undistorted pinhole
@@ -122,10 +122,18 @@ class SparseImgAlign:
         come from differently calibrated cameras (plsvo_align_multicam_batch_run).  sizes: with cameras, array-like
         [B, 2] of every pair's (width, height) when the pairs' frames differ in size: data.cam's size is then the slot
         each pair's frames sit in, top-left (synth.merge_sizes builds such a batch); data.cam's size for every pair
-        when None."""
-        _one_camera_model(camera, cameras, sizes)
+        when None.  cam_of_pair: [B] indices into `camera`, then a sequence of ATANCamera, when the pairs come from
+        differently calibrated ATAN cameras (plsvo_align_atan_multicam_batch_run): pair b is aligned with
+        camera[cam_of_pair[b]], its frames that camera's size in the top-left corner of data.cam's slot."""
+        atan_cams = _atan_cameras_arg(camera, cameras, sizes, cam_of_pair, data)
         batch, keep = abi.make_align_batch(data)
         out = abi.AlignOut(data.batch, data.n_segs)
+        if atan_cams is not None:
+            self.ctx.check(self.ctx.lib.plsvo_align_atan_multicam_batch_run(self.ctx.handle, atan_cams, C.byref(batch),
+                                                                            C.byref(self.params), C.byref(out.struct)),
+                           "plsvo_align_atan_multicam_batch_run")
+            self.last = out
+            return out
         if cameras is not None:
             cams = _cameras_arg(cameras, data, sizes)
             self.ctx.check(self.ctx.lib.plsvo_align_multicam_batch_run(self.ctx.handle, cams, C.byref(batch),
@@ -203,7 +211,7 @@ class pose_optimizer:
 
 def track(align_data, poseopt_data, max_level: int = 4, min_level: int = 2, n_iter: int = 30, reproj_thresh: float = 2.0,
           po_n_iter: int = 10, po_n_iter_ref: int | None = None, chained: bool = True, ctx: Context | None = None,
-          camera: "ATANCamera | None" = None, cameras=None, sizes=None):
+          camera: "ATANCamera | None" = None, cameras=None, sizes=None, cam_of_pair=None):
     """FrameHandlerMono::processFrame's two hot-path calls back to back (src/frame_handler_mono.cpp:272-274, :327-329):
     SparseImgAlign::run on every pair, then pose_optimizer::optimizeGaussNewton on every frame, the pose staying on the
     device in between (chained=True: the pose optimiser starts from the aligned pose of the same batch index).
@@ -211,8 +219,11 @@ def track(align_data, poseopt_data, max_level: int = 4, min_level: int = 2, n_it
     errorMultiplier2().  cameras: array-like [B, 4] of per-pair undistorted pinhole (fx, fy, cx, cy)
     (plsvo_track_multicam_batch_run); frame b's errorMultiplier2 is then |cameras[b, 0]| and poseopt_data.fx is not used.
     sizes: with cameras, [B, 2] of every pair's (width, height), as for SparseImgAlign.run.
+    cam_of_pair: with a sequence of ATANCamera as `camera`, as for SparseImgAlign.run
+    (plsvo_track_atan_multicam_batch_run); frame b's errorMultiplier2 is then its camera's fx_ and poseopt_data.fx is
+    not used.
     Returns (AlignOut, PoseOptOut)."""
-    _one_camera_model(camera, cameras, sizes)
+    atan_cams = _atan_cameras_arg(camera, cameras, sizes, cam_of_pair, align_data)
     ctx = ctx or default_context()
     ap = abi.align_params(max_level, min_level, n_iter)
     pp = abi.poseopt_params(reproj_thresh, po_n_iter, -1 if po_n_iter_ref is None else po_n_iter_ref)
@@ -222,6 +233,11 @@ def track(align_data, poseopt_data, max_level: int = 4, min_level: int = 2, n_it
         pb.T_f_w = abi._f64p()
     ao = abi.AlignOut(align_data.batch, align_data.n_segs)
     po = abi.PoseOptOut(poseopt_data.batch, poseopt_data.n_pts, poseopt_data.n_segs)
+    if atan_cams is not None:
+        ctx.check(ctx.lib.plsvo_track_atan_multicam_batch_run(ctx.handle, atan_cams, C.byref(ab), C.byref(ap), C.byref(pb),
+                                                              C.byref(pp), C.byref(ao.struct), C.byref(po.struct)),
+                  "plsvo_track_atan_multicam_batch_run")
+        return ao, po
     if cameras is not None:
         cams = _cameras_arg(cameras, align_data, sizes)
         ctx.check(ctx.lib.plsvo_track_multicam_batch_run(ctx.handle, cams, C.byref(ab), C.byref(ap), C.byref(pb), C.byref(pp),
@@ -244,6 +260,24 @@ def _one_camera_model(camera, cameras, sizes=None):
         raise PlsvoError("pass camera= (one ATAN camera) or cameras= (pinhole intrinsics per pair), not both")
     if sizes is not None and cameras is None:
         raise PlsvoError("sizes= needs cameras= (the pinhole intrinsics of every pair)")
+
+
+def _atan_cameras_arg(camera, cameras, sizes, cam_of_pair, data):
+    """plsvo_atan_camera[B] of the ATAN multicam calls when `camera` is a sequence of ATANCamera indexed by cam_of_pair;
+    None for the other camera arguments, which _one_camera_model checks."""
+    if cam_of_pair is None:
+        _one_camera_model(camera, cameras, sizes)
+        if isinstance(camera, (list, tuple)):
+            raise PlsvoError("camera= is one ATANCamera; a sequence of them needs cam_of_pair=")
+        return None
+    if cameras is not None or sizes is not None:
+        raise PlsvoError("cam_of_pair= selects ATAN cameras per pair: pass no cameras= or sizes= with it")
+    if isinstance(camera, ATANCamera) or not isinstance(camera, (list, tuple)) or not all(isinstance(c, ATANCamera) for c in camera):
+        raise PlsvoError("with cam_of_pair, camera must be a sequence of ATANCamera")
+    try:
+        return abi.make_atan_cameras([c.struct for c in camera], cam_of_pair, data.batch)
+    except ValueError as e:
+        raise PlsvoError(str(e)) from None
 
 
 def _cameras_arg(cameras, data, sizes=None):
@@ -392,7 +426,7 @@ class PinholeCamera:
 class ATANCamera:
     """vk::ATANCamera(width, height, fx, fy, cx, cy, d0), the FOV model (fx..cy normalised by the image size), as
     app/run_pipeline.cpp builds it for cam_model ATAN.  Frames from it are aligned and tracked without rectification:
-    pass it as `camera=` to SparseImgAlign.run and track.  world2cam / cam2world / errorMultiplier2 restate the model in
+    pass it as `camera=` to SparseImgAlign.run and track (a sequence of them with cam_of_pair= for one camera per pair).  world2cam / cam2world / errorMultiplier2 restate the model in
     NumPy (float64, the constructor's derived members and operation order; include/plsvo_b200.h states the formulas)."""
 
     def __init__(self, width: int, height: int, fx: float, fy: float, cx: float, cy: float, d0: float):

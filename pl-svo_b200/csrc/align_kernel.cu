@@ -222,17 +222,27 @@ struct AtanCam {  // vk::ATANCamera, the FOV model (oracle/refdeps/vikit/atan_ca
 struct PinholePerPair {  // vk::PinholeCamera without distortion, one per pair
   static constexpr bool kAtan = false, kPerPair = true;
 };
+struct AtanPerPair {  // vk::ATANCamera, one per pair: fx_..cy_ from a.cams[b], s_, s_inv_, tans_, tans_inv_ from a.atan_terms
+  static constexpr bool kAtan = true, kPerPair = true;
+};
 
-// fx, fy, cx, cy of the CTA's current pair (PinholePerPair only), then its frame's width and height as two int32 in
-// K[4]: static shared memory, which only the PinholePerPair kernels instantiate.  The 40 bytes cost 128 per CTA (the
-// dynamic region behind them is 128-byte aligned); the host plan reads the compiled size through
-// align_multicam_kernel_static_smem.  Thread 0 fills it from a.cams when the pair starts; every use reads it back, as the
-// pass reads ctl->dscale, so the intrinsics and the size take no registers across the pass.
+// fx, fy, cx, cy of the CTA's current pair (the per-pair cameras only), then its frame's width and height as two int32
+// in K[4], then (AtanPerPair) its distortion terms s_, s_inv_, tans_, tans_inv_ in K[5..8]: static shared memory, which
+// only the per-pair kernels instantiate.  The 40 (ATAN: 72) bytes cost 128 per CTA (the dynamic region behind them is
+// 128-byte aligned); the host plan reads the compiled size through align_multicam_kernel_static_smem /
+// align_atan_multicam_kernel_static_smem.  Thread 0 fills it from a.cams (and a.atan_terms) when the pair starts; every
+// use reads it back, as the pass reads ctl->dscale, so the camera and the size take no registers across the pass.
 template <class Cam>
 __device__ __forceinline__ double* pair_intrinsics() {
   static_assert(Cam::kPerPair, "only the per-pair camera keeps its intrinsics in shared memory");
-  __shared__ double K[5];
+  __shared__ double K[Cam::kAtan ? 9 : 5];
   return K;
+}
+// s_, s_inv_, tans_, tans_inv_ of the CTA's current pair (AtanPerPair only)
+template <class Cam>
+__device__ __forceinline__ const double* pair_atan_terms() {
+  static_assert(Cam::kAtan && Cam::kPerPair, "only the per-pair ATAN camera keeps its distortion terms in shared memory");
+  return pair_intrinsics<Cam>() + 5;
 }
 // The pair's frame size (width, height): the top-left corner of the batch's a.width x a.height slot it sits in.
 template <class Cam>
@@ -255,8 +265,10 @@ __device__ __forceinline__ void cam2world(const AlignArgs& a, const double* px, 
     x = __ddiv_rn(__dsub_rn(px[0], a.cx), a.fx), y = __ddiv_rn(__dsub_rn(px[1], a.cy), a.fy);
   }
   if constexpr (Cam::kAtan) {
+    double s = a.atan_s, tans_inv = a.atan_tans_inv;
+    if constexpr (Cam::kPerPair) s = pair_atan_terms<Cam>()[0], tans_inv = pair_atan_terms<Cam>()[3];
     const double rd = __dsqrt_rn(__dadd_rn(__dmul_rn(x, x), __dmul_rn(y, y)));
-    const double r = a.atan_s != 0.0 ? __dmul_rn(tan(__dmul_rn(rd, a.atan_s)), a.atan_tans_inv) : rd;
+    const double r = s != 0.0 ? __dmul_rn(tan(__dmul_rn(rd, s)), tans_inv) : rd;
     const double factor = rd > 0.01 ? __ddiv_rn(r, rd) : 1.0;
     x = __dmul_rn(factor, x), y = __dmul_rn(factor, y);
   }
@@ -317,7 +329,16 @@ __device__ __forceinline__ void project(const PairCtl* ctl, const AlignArgs& a, 
   const double yc = R[3] * xn + R[4] * yn + (R[5] + t[1] * zi);
   const double zc = R[6] * xn + R[7] * yn + (R[8] + t[2] * zi);
   const double izc = __drcp_rn(zc);
-  if constexpr (Cam::kAtan) {
+  if constexpr (Cam::kAtan && Cam::kPerPair) {
+    const double* K = pair_intrinsics<Cam>();
+    const double* T = pair_atan_terms<Cam>();
+    const double un = xc * izc, vn = yc * izc;
+    const double r = __dsqrt_rn(__dadd_rn(__dmul_rn(un, un), __dmul_rn(vn, vn)));
+    double factor = 1.0;
+    if (!(r < 0.001) && T[0] != 0.0) factor = __ddiv_rn(__dmul_rn(T[1], atan(__dmul_rn(r, T[2]))), r);
+    u = __dadd_rn(K[2], __dmul_rn(K[0], __dmul_rn(factor, un))) * ctl->dscale;
+    v = __dadd_rn(K[3], __dmul_rn(K[1], __dmul_rn(factor, vn))) * ctl->dscale;
+  } else if constexpr (Cam::kAtan) {
     const double un = xc * izc, vn = yc * izc;
     const double r = __dsqrt_rn(__dadd_rn(__dmul_rn(un, un), __dmul_rn(vn, vn)));
     double factor = 1.0;
@@ -761,6 +782,8 @@ __device__ __forceinline__ void align_pairs(const AlignArgs& a) {
         const plsvo_camera& cam = a.cams[b];
         K[0] = cam.fx, K[1] = cam.fy, K[2] = cam.cx, K[3] = cam.cy;
         pair_size<Cam>()[0] = cam.width, pair_size<Cam>()[1] = cam.height;
+        if constexpr (Cam::kAtan)
+          for (int i = 0; i < 4; ++i) K[5 + i] = a.atan_terms[4 * (size_t)b + i];
       }
     }
     // Host-buffer pipeline with lean inputs: pyramid levels above a.derive_from were not shipped; this CTA forms them
@@ -1410,6 +1433,11 @@ __global__ void __launch_bounds__(NT, MINB) sparse_img_align_multicam_kernel(con
   align_pairs<NT, PinholePerPair>(a);
 }
 
+template <int NT, int MINB>
+__global__ void __launch_bounds__(NT, MINB) sparse_img_align_atan_multicam_kernel(const AlignArgs a) {
+  align_pairs<NT, AtanPerPair>(a);
+}
+
 }  // namespace
 
 namespace {
@@ -1558,6 +1586,54 @@ cudaError_t align_multicam_kernel_launch(const AlignArgs& a, int grid, int threa
   if (threads == NT && min_blocks == MB) {                                     \
     sparse_img_align_multicam_kernel<NT, MB><<<grid, NT, smem_bytes, s>>>(a);  \
     return cudaGetLastError();                                                 \
+  }
+  PLSVO_ALIGN_VARIANTS(X)
+#undef X
+  return cudaErrorInvalidValue;
+}
+
+// the same variants with a vk::ATANCamera per pair (a.cams, a.atan_terms)
+namespace {
+template <int NT, int MINB>
+cudaError_t prepare_atan_multicam_t(size_t smem_bytes, int* ctas_per_sm) {
+  cudaError_t e = cudaFuncSetAttribute(sparse_img_align_atan_multicam_kernel<NT, MINB>,
+                                       cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_bytes);
+  if (e != cudaSuccess) return e;
+  e = cudaFuncSetAttribute(sparse_img_align_atan_multicam_kernel<NT, MINB>, cudaFuncAttributePreferredSharedMemoryCarveout,
+                           cudaSharedmemCarveoutMaxShared);
+  if (e != cudaSuccess) return e;
+  return cudaOccupancyMaxActiveBlocksPerMultiprocessor(ctas_per_sm, sparse_img_align_atan_multicam_kernel<NT, MINB>, NT,
+                                                       smem_bytes);
+}
+}  // namespace
+
+cudaError_t align_atan_multicam_kernel_prepare(int threads, int min_blocks, size_t smem_bytes, int* ctas_per_sm) {
+#define X(NT, MB) \
+  if (threads == NT && min_blocks == MB) return prepare_atan_multicam_t<NT, MB>(smem_bytes, ctas_per_sm);
+  PLSVO_ALIGN_VARIANTS(X)
+#undef X
+  return cudaErrorInvalidValue;
+}
+
+cudaError_t align_atan_multicam_kernel_static_smem(int threads, int min_blocks, size_t* bytes) {
+  cudaFuncAttributes fa;
+#define X(NT, MB)                                                                                \
+  if (threads == NT && min_blocks == MB) {                                                       \
+    const cudaError_t e = cudaFuncGetAttributes(&fa, sparse_img_align_atan_multicam_kernel<NT, MB>); \
+    *bytes = e == cudaSuccess ? fa.sharedSizeBytes : 0;                                          \
+    return e;                                                                                    \
+  }
+  PLSVO_ALIGN_VARIANTS(X)
+#undef X
+  return cudaErrorInvalidValue;
+}
+
+cudaError_t align_atan_multicam_kernel_launch(const AlignArgs& a, int grid, int threads, int min_blocks, size_t smem_bytes,
+                                              cudaStream_t s) {
+#define X(NT, MB)                                                                   \
+  if (threads == NT && min_blocks == MB) {                                          \
+    sparse_img_align_atan_multicam_kernel<NT, MB><<<grid, NT, smem_bytes, s>>>(a);  \
+    return cudaGetLastError();                                                      \
   }
   PLSVO_ALIGN_VARIANTS(X)
 #undef X

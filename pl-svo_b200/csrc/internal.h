@@ -72,6 +72,9 @@ struct AlignArgs {
   double atan_s, atan_s_inv, atan_tans, atan_tans_inv;
   // [B] camera of every pair (the multicam kernels read its fx, fy, cx, cy instead of fx, fy, cx, cy above)
   const plsvo_camera* cams;
+  // [B][4] s_, s_inv_, tans_, tans_inv_ of every pair's vk::ATANCamera (read by the ATAN multicam kernels only, instead
+  // of atan_s..atan_tans_inv above; a.cams[b] then holds the pair's members fx_, fy_, cx_, cy_ and its size)
+  const double* atan_terms;
 };
 
 // Opaque chi2 patches (16 float terms each) the alignment kernel can hold per Gauss-Newton pass: the patches whose 16
@@ -105,6 +108,14 @@ __attribute__((weak)) cudaError_t align_multicam_kernel_prepare(int threads, int
                                                                 int* ctas_per_sm);
 __attribute__((weak)) cudaError_t align_multicam_kernel_launch(const AlignArgs& a, int grid, int threads, int min_blocks,
                                                                size_t smem_bytes, cudaStream_t s);
+// The same kernel variants with a vk::ATANCamera per pair, AlignArgs::cams and AlignArgs::atan_terms
+// (plsvo_align_atan_multicam_batch_run).  Weak for the same reason; their static shared memory (the pair's members, size
+// and distortion terms, 72 bytes padded to 128 on sm_90a) is reported and planned for as for the multicam kernels.
+__attribute__((weak)) cudaError_t align_atan_multicam_kernel_static_smem(int threads, int min_blocks, size_t* bytes);
+__attribute__((weak)) cudaError_t align_atan_multicam_kernel_prepare(int threads, int min_blocks, size_t smem_bytes,
+                                                                     int* ctas_per_sm);
+__attribute__((weak)) cudaError_t align_atan_multicam_kernel_launch(const AlignArgs& a, int grid, int threads, int min_blocks,
+                                                                    size_t smem_bytes, cudaStream_t s);
 
 // ---------------------------------------------------------------------------------------------
 struct PoseOptArgs {

@@ -67,6 +67,7 @@ struct plsvo_ctx_impl {
   bool atan = false;               // the uploaded batch is seen through a vk::ATANCamera (the ATAN kernel variants)
   bool multicam = false;           // every pair has its own pinhole intrinsics, aa.cams (the multicam kernel variants)
   DevBuf d_cams;                   // plsvo_camera[B] of a multicam batch
+  DevBuf d_atan_terms;             // [B][4] distortion terms of an ATAN multicam batch (aa.atan_terms)
   DevBuf d_feat;                     // every per-pair input array of the batch, at 256-byte-aligned offsets
   size_t feat_bytes = 0;
   char* h_po_out = nullptr;          // pinned staging of the pose-optimiser outputs (one D2H per download)
@@ -104,7 +105,8 @@ struct plsvo_ctx_impl {
     DevBuf map1, map2;
   };
   std::vector<std::unique_ptr<CamMap>> mc_maps;
-  std::vector<plsvo_camera> h_mc_cams;  // plsvo_camera[B] of a raw multicam call, staged for multicam_select
+  std::vector<plsvo_camera> h_mc_cams;  // plsvo_camera[B] of a raw or ATAN multicam call, staged for multicam_select
+  std::vector<double> h_atan_terms;     // [B][4] distortion terms of an ATAN multicam call, staged for the upload
   std::vector<RawVisit> h_visit;        // the frames of a raw multicam call in camera-grouped order, with their maps
   DevBuf d_visit;
   DevBuf p_out_T;  // every pose-optimiser output, one block
@@ -374,6 +376,7 @@ int align_layout(plsvo_ctx_impl* c, const plsvo_align_batch* h) {
   c->atan = false;  // the ATAN entry points set it after the upload
   c->multicam = false;  // and so do the multicam entry points
   a.cams = nullptr;
+  a.atan_terms = nullptr;
   a.B = h->batch, a.n_pts = h->n_pts, a.n_segs = h->n_segs;
   a.width = h->cam.width, a.height = h->cam.height;
   a.fx = h->cam.fx, a.fy = h->cam.fy, a.cx = h->cam.cx, a.cy = h->cam.cy;
@@ -821,10 +824,12 @@ int align_plan(plsvo_ctx_impl* c, const plsvo_align_params* p, AlignPlan* plan, 
       rc_last = fail(c, PLSVO_ERR_INVALID, "a segment has more than 1024 samples");
       continue;
     }
-    // static shared memory of the kernel, taken per CTA next to the dynamic plan below: the multicam kernels hold
-    // their pair's intrinsics there (with the alignment of the dynamic region behind them); the others have none
+    // static shared memory of the kernel, taken per CTA next to the dynamic plan below: the multicam kernels (pinhole
+    // and ATAN) hold their pair's camera there (with the alignment of the dynamic region behind them); the others have none
     size_t static_smem = 0;
-    if (c->multicam) CK(align_multicam_kernel_static_smem(threads, min_blocks, &static_smem));
+    if (c->multicam)
+      CK(c->atan ? align_atan_multicam_kernel_static_smem(threads, min_blocks, &static_smem)
+                 : align_multicam_kernel_static_smem(threads, min_blocks, &static_smem));
     // shared-memory plan: stage the current image level when the CTA still fits min_blocks times per SM next to
     // the per-pair state; bigger levels are read through L2 with the same aligned-word loads.
     const int other = (int)(align_smem_bytes(a.n_pts, a.n_segs, a.max_patches, a.max_seg_slots, 0, threads) + static_smem);
@@ -857,9 +862,10 @@ int align_plan(plsvo_ctx_impl* c, const plsvo_align_params* p, AlignPlan* plan, 
     a.smem_img_bytes = img_bytes;
     a.rec_cap = rec_cap;
     int ctas_per_sm = 0;
-    CK(c->atan       ? align_atan_kernel_prepare(threads, min_blocks, smem, &ctas_per_sm)
-       : c->multicam ? align_multicam_kernel_prepare(threads, min_blocks, smem, &ctas_per_sm)
-                     : align_kernel_prepare(threads, min_blocks, smem, &ctas_per_sm));
+    CK(c->atan && c->multicam ? align_atan_multicam_kernel_prepare(threads, min_blocks, smem, &ctas_per_sm)
+       : c->atan              ? align_atan_kernel_prepare(threads, min_blocks, smem, &ctas_per_sm)
+       : c->multicam          ? align_multicam_kernel_prepare(threads, min_blocks, smem, &ctas_per_sm)
+                              : align_kernel_prepare(threads, min_blocks, smem, &ctas_per_sm));
     if (ctas_per_sm < 1) {
       rc_last = fail(c, PLSVO_ERR_INVALID, "kernel does not fit on an SM");
       continue;
@@ -896,9 +902,10 @@ int align_launch_kernel(plsvo_ctx_impl* c, const AlignPlan& plan, cudaStream_t s
   a.gate_chunk = gate_chunk;
   const int grid = std::min(a.B, c->num_sms * plan.ctas_per_sm);
   CK(cudaMemsetAsync(a.work_counter, 0, sizeof(unsigned int), s));
-  CK(c->atan       ? align_atan_kernel_launch(a, grid, plan.threads, plan.min_blocks, plan.smem, s)
-     : c->multicam ? align_multicam_kernel_launch(a, grid, plan.threads, plan.min_blocks, plan.smem, s)
-                   : align_kernel_launch(a, grid, plan.threads, plan.min_blocks, plan.smem, s));
+  CK(c->atan && c->multicam ? align_atan_multicam_kernel_launch(a, grid, plan.threads, plan.min_blocks, plan.smem, s)
+     : c->atan              ? align_atan_kernel_launch(a, grid, plan.threads, plan.min_blocks, plan.smem, s)
+     : c->multicam          ? align_multicam_kernel_launch(a, grid, plan.threads, plan.min_blocks, plan.smem, s)
+                            : align_kernel_launch(a, grid, plan.threads, plan.min_blocks, plan.smem, s));
   c->launches += 1;
   return PLSVO_OK;
 }
@@ -1298,38 +1305,47 @@ int plsvo_poseopt_batch_run(plsvo_ctx* ctx, const plsvo_poseopt_batch* b, const 
 // ------------------------------------------------------------------------------------------------
 namespace {
 
+// vk::ATANCamera's constructor: the members of `cam` — its size and fx_, fy_, cx_, cy_ as a plsvo_camera record (what the
+// kernels read as fx, fy, cx, cy), and its distortion terms s_, s_inv_, tans_, tans_inv_ (all zero but s_ when s_ == 0).
+// The uniform and the per-pair ATAN calls both derive them here, so they compute the same bits.  Returns nullptr, or what
+// is wrong with the camera.
+const char* atan_members(const plsvo_atan_camera& cam, plsvo_camera* k, double terms[4]) {
+  if (!std::isfinite(cam.fx) || !std::isfinite(cam.fy) || !std::isfinite(cam.cx) || !std::isfinite(cam.cy) || !std::isfinite(cam.d0))
+    return "has a non-finite parameter";
+  if (!(cam.fx > 0.0) || !(cam.fy > 0.0)) return "fx and fy must be positive";
+  *k = plsvo_camera{cam.width, cam.height, 0, 0, (double)cam.width * cam.fx, (double)cam.height * cam.fy,
+                    cam.cx * (double)cam.width - 0.5, cam.cy * (double)cam.height - 0.5};
+  if (!std::isfinite(k->fx) || !std::isfinite(k->fy) || !(k->fx > 0.0) || !(k->fy > 0.0)) return "focal length out of range";
+  terms[0] = cam.d0;
+  terms[1] = terms[2] = terms[3] = 0.0;
+  if (cam.d0 != 0.0) {
+    terms[2] = 2.0 * tan(cam.d0 / 2.0);
+    terms[3] = 1.0 / terms[2];
+    terms[1] = 1.0 / cam.d0;
+  }
+  return nullptr;
+}
+
 // Validates the camera against the batch and returns in *derived the batch with cam.fx / fy / cx / cy replaced by the
-// ATANCamera members fx_, fy_, cx_, cy_ (what the kernels read as fx, fy, cx, cy).  Nothing is queued here.
-int atan_batch(plsvo_ctx_impl* c, const plsvo_atan_camera* cam, const plsvo_align_batch* b, plsvo_align_batch* derived) {
+// ATANCamera members fx_, fy_, cx_, cy_, and in terms[4] its distortion terms.  Nothing is queued here.
+int atan_batch(plsvo_ctx_impl* c, const plsvo_atan_camera* cam, const plsvo_align_batch* b, plsvo_align_batch* derived,
+               double terms[4]) {
   if (cam->width != b->cam.width || cam->height != b->cam.height)
     return fail(c, PLSVO_ERR_INVALID, "plsvo_atan_camera size differs from batch->cam");
-  if (!std::isfinite(cam->fx) || !std::isfinite(cam->fy) || !std::isfinite(cam->cx) || !std::isfinite(cam->cy) ||
-      !std::isfinite(cam->d0))
-    return fail(c, PLSVO_ERR_INVALID, "plsvo_atan_camera has a non-finite parameter");
-  if (!(cam->fx > 0.0) || !(cam->fy > 0.0)) return fail(c, PLSVO_ERR_INVALID, "plsvo_atan_camera fx and fy must be positive");
+  plsvo_camera k;
+  if (const char* why = atan_members(*cam, &k, terms)) return fail(c, PLSVO_ERR_INVALID, (std::string("plsvo_atan_camera ") + why).c_str());
   *derived = *b;
-  derived->cam.fx = (double)cam->width * cam->fx;
-  derived->cam.fy = (double)cam->height * cam->fy;
-  derived->cam.cx = cam->cx * (double)cam->width - 0.5;
-  derived->cam.cy = cam->cy * (double)cam->height - 0.5;
-  if (!std::isfinite(derived->cam.fx) || !std::isfinite(derived->cam.fy) || !(derived->cam.fx > 0.0) || !(derived->cam.fy > 0.0))
-    return fail(c, PLSVO_ERR_INVALID, "plsvo_atan_camera focal length out of range");
+  derived->cam.fx = k.fx, derived->cam.fy = k.fy, derived->cam.cx = k.cx, derived->cam.cy = k.cy;
   if (!align_atan_kernel_prepare || !align_atan_kernel_launch)
     return fail(c, PLSVO_ERR_CUDA, "this library was built without the ATAN alignment kernels");
   return PLSVO_OK;
 }
 
 // after the upload of the derived batch: select the ATAN kernels and give them the distortion terms of the constructor
-void atan_select(plsvo_ctx_impl* c, const plsvo_atan_camera* cam) {
+void atan_select(plsvo_ctx_impl* c, const double terms[4]) {
   AlignArgs& a = c->aa;
   c->atan = true;
-  a.atan_s = cam->d0;
-  a.atan_s_inv = a.atan_tans = a.atan_tans_inv = 0.0;
-  if (cam->d0 != 0.0) {
-    a.atan_tans = 2.0 * tan(cam->d0 / 2.0);
-    a.atan_tans_inv = 1.0 / a.atan_tans;
-    a.atan_s_inv = 1.0 / cam->d0;
-  }
+  a.atan_s = terms[0], a.atan_s_inv = terms[1], a.atan_tans = terms[2], a.atan_tans_inv = terms[3];
 }
 
 }  // namespace
@@ -1340,10 +1356,11 @@ static int align_atan_body(plsvo_ctx* ctx, const plsvo_atan_camera* cam, const p
                            const plsvo_align_result* o) {
   plsvo_ctx_impl* c = CTX(ctx);
   plsvo_align_batch d;
-  int rc = atan_batch(c, cam, b, &d);
+  double terms[4];
+  int rc = atan_batch(c, cam, b, &d, terms);
   if (rc == PLSVO_OK) rc = plsvo_align_upload(ctx, &d);
   if (rc != PLSVO_OK) return rc;
-  atan_select(c, cam);
+  atan_select(c, terms);
   rc = plsvo_align_launch(ctx, p);
   if (rc == PLSVO_OK) rc = plsvo_align_download(ctx, o);
   return rc;
@@ -1360,10 +1377,11 @@ static int track_atan_body(plsvo_ctx* ctx, const plsvo_atan_camera* cam, const p
                            const plsvo_poseopt_result* po) {
   plsvo_ctx_impl* c = CTX(ctx);
   plsvo_align_batch d;
-  int rc = atan_batch(c, cam, ab, &d);
+  double terms[4];
+  int rc = atan_batch(c, cam, ab, &d, terms);
   if (rc == PLSVO_OK) rc = plsvo_track_upload(ctx, &d, pb);
   if (rc != PLSVO_OK) return rc;
-  atan_select(c, cam);
+  atan_select(c, terms);
   rc = plsvo_track_launch(ctx, ap, pp);
   if (rc == PLSVO_OK && ao) rc = plsvo_align_download(ctx, ao);
   if (rc == PLSVO_OK) rc = plsvo_poseopt_download(ctx, po);
@@ -1396,19 +1414,25 @@ int level_under_one_pixel(int w, int h, const plsvo_align_batch* b, int max_leve
   return -1;
 }
 
+// cams[i], of size w x h, against the slot (batch->cam's size): at least one pixel and no wider or taller than the slot
+int camera_fits_slot(plsvo_ctx_impl* c, int i, int w, int h, const plsvo_align_batch* b) {
+  if (w >= 1 && h >= 1 && w <= b->cam.width && h <= b->cam.height) return PLSVO_OK;
+  char msg[192];
+  snprintf(msg, sizeof msg, "cams[%d] is %dx%d, batch->cam is %dx%d: every camera must fit inside the batch's image slot", i, w, h,
+           b->cam.width, b->cam.height);
+  return fail(c, PLSVO_ERR_INVALID, msg);
+}
+
 // cams[0..B) against the batch: a size that fits the slot (batch->cam's size) and whose levels are at least one pixel,
-// finite intrinsics, fx and fy non-zero; in a frame chain, consecutive pairs share a frame and so a size.  Nothing is
-// queued here.
+// finite intrinsics, fx and fy non-zero; in a frame chain, consecutive pairs share a frame and so a size.  A batch of
+// no pairs or fewer is rejected here, before the callers size their per-pair host arrays by it.  Nothing is queued here.
 int multicam_check(plsvo_ctx_impl* c, const plsvo_camera* cams, const plsvo_align_batch* b, const plsvo_align_params* p) {
   if (!cams) return fail(c, PLSVO_ERR_INVALID, "cams is NULL");
+  if (b->batch <= 0) return fail(c, PLSVO_ERR_INVALID, "batch/n_pts/n_segs out of range");
   char msg[192];
   for (int i = 0; i < b->batch; ++i) {
     const plsvo_camera& k = cams[i];
-    if (k.width < 1 || k.height < 1 || k.width > b->cam.width || k.height > b->cam.height) {
-      snprintf(msg, sizeof msg, "cams[%d] is %dx%d, batch->cam is %dx%d: every camera must fit inside the batch's image slot", i,
-               k.width, k.height, b->cam.width, b->cam.height);
-      return fail(c, PLSVO_ERR_INVALID, msg);
-    }
+    if (camera_fits_slot(c, i, k.width, k.height, b) != PLSVO_OK) return PLSVO_ERR_INVALID;
     const int l = k.width == b->cam.width && k.height == b->cam.height ? -1 : level_under_one_pixel(k.width, k.height, b, p->max_level);
     if (l >= 0) {
       snprintf(msg, sizeof msg, "cams[%d] is %dx%d: pyramid level %d smaller than one pixel", i, k.width, k.height, l);
@@ -1533,6 +1557,98 @@ int plsvo_track_multicam_batch_run(plsvo_ctx* ctx, const plsvo_camera* cams, con
                                    const plsvo_poseopt_result* po) {
   if (!ctx || !ab || !ap || !pb || !pp || !po) return PLSVO_ERR_INVALID;
   return settled(CTX(ctx), track_multicam_body(ctx, cams, ab, ap, pb, pp, ao, po));
+}
+
+}  // extern "C"
+
+// ------------------------------------------------------------------------------------------------
+// Multicam ATAN batches: a vk::ATANCamera per pair, in slots of batch->cam's size
+// ------------------------------------------------------------------------------------------------
+namespace {
+
+// cams[0..B) of an ATAN multicam call: every camera's members into c->h_mc_cams (plsvo_camera records) and its distortion
+// terms into c->h_atan_terms ([B][4]), then the multicam rules on the records (slot, size, levels, frame chains).
+// Nothing is queued here.
+int atan_multicam_check(plsvo_ctx_impl* c, const plsvo_atan_camera* cams, const plsvo_align_batch* b, const plsvo_align_params* p) {
+  if (!cams) return fail(c, PLSVO_ERR_INVALID, "cams is NULL");
+  if (b->batch <= 0) return fail(c, PLSVO_ERR_INVALID, "batch/n_pts/n_segs out of range");
+  const size_t B = (size_t)b->batch;
+  c->h_mc_cams.resize(B);
+  c->h_atan_terms.resize(4 * B);
+  for (size_t i = 0; i < B; ++i) {
+    // the size first: the derived focal lengths of a camera below one pixel would be reported instead
+    if (camera_fits_slot(c, (int)i, cams[i].width, cams[i].height, b) != PLSVO_OK) return PLSVO_ERR_INVALID;
+    if (const char* why = atan_members(cams[i], &c->h_mc_cams[i], &c->h_atan_terms[4 * i])) {
+      char msg[128];
+      snprintf(msg, sizeof msg, "cams[%d] %s", (int)i, why);
+      return fail(c, PLSVO_ERR_INVALID, msg);
+    }
+  }
+  int rc = multicam_check(c, c->h_mc_cams.data(), b, p);
+  if (rc == PLSVO_OK && (!align_atan_multicam_kernel_prepare || !align_atan_multicam_kernel_launch ||
+                         !align_atan_multicam_kernel_static_smem))
+    rc = fail(c, PLSVO_ERR_CUDA, "this library was built without the ATAN multicam alignment kernels");
+  return rc;
+}
+
+// after the upload of the alignment batch: the pairs' members and distortion terms follow it on the same stream, and the
+// ATAN multicam kernels run the batch
+int atan_multicam_select(plsvo_ctx_impl* c) {
+  int rc = multicam_select(c, c->h_mc_cams.data());
+  if (rc != PLSVO_OK) return rc;
+  CK(up(c->d_atan_terms, c->h_atan_terms.data(), c->h_atan_terms.size(), c->stream, &c->aa.atan_terms));
+  c->atan = true;
+  return PLSVO_OK;
+}
+
+}  // namespace
+
+extern "C" {
+
+static int align_atan_multicam_body(plsvo_ctx* ctx, const plsvo_atan_camera* cams, const plsvo_align_batch* b,
+                                    const plsvo_align_params* p, const plsvo_align_result* o) {
+  plsvo_ctx_impl* c = CTX(ctx);
+  int rc = atan_multicam_check(c, cams, b, p);
+  if (rc == PLSVO_OK) rc = plsvo_align_upload(ctx, b);
+  if (rc == PLSVO_OK) rc = atan_multicam_select(c);
+  if (rc == PLSVO_OK) rc = plsvo_align_launch(ctx, p);
+  if (rc == PLSVO_OK) rc = plsvo_align_download(ctx, o);
+  return rc;
+}
+
+int plsvo_align_atan_multicam_batch_run(plsvo_ctx* ctx, const plsvo_atan_camera* cams, const plsvo_align_batch* b,
+                                        const plsvo_align_params* p, const plsvo_align_result* o) {
+  if (!ctx || !b || !p || !o) return PLSVO_ERR_INVALID;
+  return settled(CTX(ctx), align_atan_multicam_body(ctx, cams, b, p, o));
+}
+
+static int track_atan_multicam_body(plsvo_ctx* ctx, const plsvo_atan_camera* cams, const plsvo_align_batch* ab,
+                                    const plsvo_align_params* ap, const plsvo_poseopt_batch* pb, const plsvo_poseopt_params* pp,
+                                    const plsvo_align_result* ao, const plsvo_poseopt_result* po) {
+  plsvo_ctx_impl* c = CTX(ctx);
+  int rc = atan_multicam_check(c, cams, ab, ap);
+  if (rc == PLSVO_OK && pb->batch != ab->batch)
+    rc = fail(c, PLSVO_ERR_INVALID, "alignment and pose-optimiser batches differ in size");
+  if (rc == PLSVO_OK) rc = multicam_kernels_present(c, false, true);
+  if (rc != PLSVO_OK) return rc;
+  // the pose optimiser of frame b reads vk::ATANCamera::errorMultiplier2() = fx_ of pair b's camera
+  c->h_po_fx.resize((size_t)ab->batch);
+  for (int i = 0; i < ab->batch; ++i) c->h_po_fx[i] = c->h_mc_cams[i].fx;
+  rc = plsvo_track_upload(ctx, ab, pb);
+  if (rc == PLSVO_OK) rc = atan_multicam_select(c);
+  if (rc == PLSVO_OK) rc = poseopt_fx_select(c, c->h_po_fx.data());
+  if (rc == PLSVO_OK) rc = plsvo_track_launch(ctx, ap, pp);
+  if (rc == PLSVO_OK && ao) rc = plsvo_align_download(ctx, ao);
+  if (rc == PLSVO_OK) rc = plsvo_poseopt_download(ctx, po);
+  return rc;
+}
+
+int plsvo_track_atan_multicam_batch_run(plsvo_ctx* ctx, const plsvo_atan_camera* cams, const plsvo_align_batch* ab,
+                                        const plsvo_align_params* ap, const plsvo_poseopt_batch* pb,
+                                        const plsvo_poseopt_params* pp, const plsvo_align_result* ao,
+                                        const plsvo_poseopt_result* po) {
+  if (!ctx || !ab || !ap || !pb || !pp || !po) return PLSVO_ERR_INVALID;
+  return settled(CTX(ctx), track_atan_multicam_body(ctx, cams, ab, ap, pb, pp, ao, po));
 }
 
 }  // extern "C"

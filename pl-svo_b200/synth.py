@@ -632,6 +632,36 @@ def make_multicam_batch(cams, cam_of_pair, n_pts: int = 300, n_segs: int = 80, s
     return al, scatter_batches(po_parts, index, B), cameras
 
 
+def make_atan_multicam_batch(cams, cam_of_pair, slot: Camera | None = None, fill=0, poseopt: bool = False, n_pts: int = 300,
+                             n_segs: int = 80, seed: int = 3000, **align_kw):
+    """A batch of pairs from several ATAN (FOV) cameras (api.ATANCamera), of one size or several: pair b is rendered and its
+    features are lifted through cams[cam_of_pair[b]] (make_align_batch(atan=), make_track_batch when `poseopt`), at that
+    camera's size.  The per-camera parts are padded into one slot batch with merge_sizes (slot, fill as there).  Returns
+    (AlignData, parts, groups), or (AlignData, PoseOptData, parts, po_parts, groups) when `poseopt`: parts[i] is the
+    AlignData of camera used[i] = the i-th camera that has pairs, at its own size, and groups[i] the positions of its pairs
+    in the batch.  The pose optimiser of frame b then takes errorMultiplier2 = its camera's fx_."""
+    cam_of_pair = np.asarray(cam_of_pair)
+    groups = [np.flatnonzero(cam_of_pair == k) for k in range(len(cams))]
+    used = [k for k in range(len(cams)) if len(groups[k])]
+    al_parts, po_parts = [], []
+    for k in used:
+        a = cams[k]
+        cam = Camera(a.width, a.height, a.fx_, a.fy_, a.cx_, a.cy_)
+        kw = dict(cam=cam, batch=len(groups[k]), n_pts=n_pts, n_segs=n_segs, seed=seed + 104729 * k, atan=a, **align_kw)
+        if poseopt:
+            al, po = make_track_batch(**kw)
+            po.fx = a.errorMultiplier2()
+            po_parts.append(po)
+        else:
+            al = make_align_batch(**kw)
+        al_parts.append(al)
+    index = [groups[k] for k in used]
+    al, _ = merge_sizes(al_parts, index, slot=slot, fill=fill)
+    if not poseopt:
+        return al, al_parts, index
+    return al, scatter_batches(po_parts, index, len(cam_of_pair)), al_parts, po_parts, index
+
+
 def make_sequence(cam: Camera = VGA, n_seq: int = 4, n_frames: int = 20, n_pts: int = 300, n_segs: int = 80, seed: int = 1000,
                   device: str | torch.device = "cpu", noise_px: float = 0.3, outlier_frac: float = 0.05):
     """BASELINE config 1 / SURVEY 8d C1: n_seq independent sequences of n_frames views along the smooth trajectory
