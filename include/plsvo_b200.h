@@ -593,6 +593,26 @@ typedef struct plsvo_match_result {
 
 int plsvo_match_direct_batch_run(plsvo_ctx* ctx, const plsvo_match_batch* in, const plsvo_match_result* out);
 
+/* ---- Matcher::findMatchDirect for frames from an ATAN (FOV) camera -------------------------------
+ * plsvo_match_direct_batch_run with the keyframes and the current frames seen through vk::ATANCamera(*cam), the model of
+ * plsvo_atan_camera above (in a reference pipeline with cam_model ATAN both are the same camera object).  Of
+ * findMatchDirect only warp::getWarpMatrixAffine reads the camera model: its two cam_ref.cam2world and three
+ * cam_cur.world2cam calls use the ATAN formulas.  The in-frame test reads the image size only, and everything downstream
+ * of A_cur_ref (search level, warped patch, edgelet direction, align2D / align1D) is unchanged.
+ * - `in` is as for plsvo_match_direct_batch_run.  in->cam.width / height must equal the camera's; the other fields of
+ *   in->cam are ignored.
+ * - A size mismatch, a non-finite parameter, fx <= 0 or fy <= 0 returns PLSVO_ERR_INVALID before anything is queued, and
+ *   the context stays usable.  A library built without the ATAN matching kernel returns PLSVO_ERR_CUDA.
+ * - Exactness: the device's atan and tan may differ from glibc's by an ulp or two, so A_cur_ref agrees with the reference
+ *   to round-off (each entry within 1e-12; the entries are O(1)).  Everything downstream of A_cur_ref is exact: search
+ *   level, success and px_cur are byte for byte what the reference computes from the returned A_cur_ref.  A candidate
+ *   whose five projections call neither tan nor atan (d0 == 0, or every argument inside both cut-offs) matches the
+ *   reference byte for byte, A_cur_ref included.
+ * - Out of scope: the depth-filter seed updates (findEpipolarMatchDirect) for ATAN frames, a camera per image or per
+ *   candidate, pinhole and ATAN candidates in one call, raw frames. */
+int plsvo_match_direct_atan_batch_run(plsvo_ctx* ctx, const plsvo_atan_camera* cam, const plsvo_match_batch* in,
+                                      const plsvo_match_result* out);
+
 /* ---- Structure optimisation: Point::optimize / LineSeg::optimize (SURVEY.md §8f rank 3, "next") ---
  * Replaces, for a batch of 3D features, include/plsvo/feature3D.h:120,157 / src/feature3D_impl.cpp:36-95,
  * 97-174 as driven by FrameHandlerBase::optimizeStructure (src/frame_handler_base.cpp:202-237):

@@ -549,6 +549,7 @@ ABI_SYMBOLS = [
     ("plsvo_align2d_batch_run", C.c_int, [C.c_void_p, _P(Align2DBatch), _P(Align2DResult)]),
     ("plsvo_align1d_batch_run", C.c_int, [C.c_void_p, _P(Align1DBatch), _P(Align1DResult)]),
     ("plsvo_match_direct_batch_run", C.c_int, [C.c_void_p, _P(MatchBatch), _P(MatchResult)]),
+    ("plsvo_match_direct_atan_batch_run", C.c_int, [C.c_void_p, _P(AtanCamera), _P(MatchBatch), _P(MatchResult)]),
     ("plsvo_seed_update_batch_run", C.c_int, [C.c_void_p, _P(SeedBatch), _P(SeedResult)]),
     ("plsvo_line_seed_update_batch_run", C.c_int, [C.c_void_p, _P(LineSeedBatch), _P(LineSeedResult)]),
     ("plsvo_structopt_batch_run", C.c_int, [C.c_void_p, _P(StructOptBatch), _P(StructOptResult)]),

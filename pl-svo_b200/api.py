@@ -426,7 +426,8 @@ class PinholeCamera:
 class ATANCamera:
     """vk::ATANCamera(width, height, fx, fy, cx, cy, d0), the FOV model (fx..cy normalised by the image size), as
     app/run_pipeline.cpp builds it for cam_model ATAN.  Frames from it are aligned and tracked without rectification:
-    pass it as `camera=` to SparseImgAlign.run and track (a sequence of them with cam_of_pair= for one camera per pair).  world2cam / cam2world / errorMultiplier2 restate the model in
+    pass it as `camera=` to SparseImgAlign.run and track (a sequence of them with cam_of_pair= for one camera per pair), and
+    to Matcher.findMatchDirect.  world2cam / cam2world / errorMultiplier2 restate the model in
     NumPy (float64, the constructor's derived members and operation order; include/plsvo_b200.h states the formulas)."""
 
     def __init__(self, width: int, height: int, fx: float, fy: float, cx: float, cy: float, d0: float):
@@ -538,13 +539,23 @@ class Matcher:
         self.align_max_iter = align_max_iter  # Matcher::Options::align_max_iter
         self.ctx = ctx or default_context()
 
-    def findMatchDirect(self, data) -> abi.MatchOut:
-        """data: synth.MatchData-like batch -> px_cur (refined, level-0 pixels), success flags, search levels."""
+    def findMatchDirect(self, data, camera: "ATANCamera | None" = None) -> abi.MatchOut:
+        """data: synth.MatchData-like batch -> px_cur (refined, level-0 pixels), success flags, search levels.
+        camera: an ATANCamera when the keyframes and current frames come from one (plsvo_match_direct_atan_batch_run;
+        data.cam then only gives the image size); None for the undistorted pinhole of data.cam."""
         data.n_iter = self.align_max_iter
+        if camera is not None:
+            if not isinstance(camera, ATANCamera):
+                raise TypeError(f"findMatchDirect: camera must be an ATANCamera or None, not {type(camera).__name__}")
+            camera._check(data)
         b, keep = abi.make_match_batch(data)
         out = abi.MatchOut(data.n)
-        self.ctx.check(self.ctx.lib.plsvo_match_direct_batch_run(self.ctx.handle, C.byref(b), C.byref(out.struct)),
-                       "plsvo_match_direct_batch_run")
+        if camera is not None:
+            self.ctx.check(self.ctx.lib.plsvo_match_direct_atan_batch_run(self.ctx.handle, C.byref(camera.struct), C.byref(b),
+                                                                          C.byref(out.struct)), "plsvo_match_direct_atan_batch_run")
+        else:
+            self.ctx.check(self.ctx.lib.plsvo_match_direct_batch_run(self.ctx.handle, C.byref(b), C.byref(out.struct)),
+                           "plsvo_match_direct_batch_run")
         return out
 
 

@@ -264,8 +264,14 @@ struct MatchArgs {
   uint8_t* out_success;
   int32_t* out_level;
   double* out_A;  // [n][4] or null
+  // vk::ATANCamera distortion (read by the ATAN kernel only; fx, fy, cx, cy above then hold fx_, fy_, cx_, cy_):
+  // s_ = d0, s_inv_ = 1/s_, tans_ = 2 tan(s_/2), tans_inv_ = 1/tans_, all zero when s_ == 0
+  double atan_s, atan_s_inv, atan_tans, atan_tans_inv;
 };
 cudaError_t match_direct_kernel_launch(const MatchArgs& a, cudaStream_t s);
+// The same kernel with the vk::ATANCamera warp matrix (plsvo_match_direct_atan_batch_run).  Weak, as the ATAN alignment
+// launchers: the host-pipeline model of the tests need not provide it, and the ATAN entry point then reports it missing.
+__attribute__((weak)) cudaError_t match_direct_atan_kernel_launch(const MatchArgs& a, cudaStream_t s);
 
 // ---------------------------------------------------------------------------------------------
 struct SeedArgs {

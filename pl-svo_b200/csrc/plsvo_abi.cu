@@ -1819,8 +1819,19 @@ int stage_pyramid(plsvo_ctx_impl* c, DevBuf& buf, const uint8_t* const* img, con
 }
 }  // namespace
 
-static int match_direct_batch_run_body(plsvo_ctx* ctx, const plsvo_match_batch* in, const plsvo_match_result* out) {
+// atan: NULL for the undistorted pinhole of in->cam, or the vk::ATANCamera both frames are seen through
+// (plsvo_match_direct_atan_batch_run); it is validated, and the kernel's presence checked, before anything is queued.
+static int match_direct_batch_run_body(plsvo_ctx* ctx, const plsvo_match_batch* in, const plsvo_match_result* out,
+                                       const plsvo_atan_camera* atan = nullptr) {
   plsvo_ctx_impl* c = CTX(ctx);
+  plsvo_camera k = in->cam;
+  double terms[4] = {0.0, 0.0, 0.0, 0.0};
+  if (atan) {
+    if (atan->width != in->cam.width || atan->height != in->cam.height)
+      return fail(c, PLSVO_ERR_INVALID, "plsvo_atan_camera size differs from in->cam");
+    if (const char* why = atan_members(*atan, &k, terms)) return fail(c, PLSVO_ERR_INVALID, (std::string("plsvo_atan_camera ") + why).c_str());
+    if (!match_direct_atan_kernel_launch) return fail(c, PLSVO_ERR_CUDA, "this library was built without the ATAN matching kernel");
+  }
   if (in->n_features < 0 || in->n_ref_images <= 0 || in->n_cur_images <= 0 || in->cam.width <= 0 || in->cam.height <= 0 ||
       in->n_iter < 0 || in->n_pyr_levels < 1 || in->n_pyr_levels > PLSVO_MAX_LEVELS)
     return fail(c, PLSVO_ERR_INVALID, "match batch description");
@@ -1844,7 +1855,8 @@ static int match_direct_batch_run_body(plsvo_ctx* ctx, const plsvo_match_batch* 
   memset(&a, 0, sizeof a);
   a.n = in->n_features, a.n_iter = in->n_iter, a.n_pyr_levels = in->n_pyr_levels;
   a.width = in->cam.width, a.height = in->cam.height;
-  a.fx = in->cam.fx, a.fy = in->cam.fy, a.cx = in->cam.cx, a.cy = in->cam.cy;
+  a.fx = k.fx, a.fy = k.fy, a.cx = k.cx, a.cy = k.cy;
+  a.atan_s = terms[0], a.atan_s_inv = terms[1], a.atan_tans = terms[2], a.atan_tans_inv = terms[3];
   int rc = stage_pyramid(c, c->m_ref_img, in->ref_img, in->ref_pitch, in->ref_stride, in->n_ref_images, a.width, a.height, s, a.ref_img,
                          a.ref_pitch, a.ref_stride);
   if (rc != PLSVO_OK) return rc;
@@ -1875,7 +1887,7 @@ static int match_direct_batch_run_body(plsvo_ctx* ctx, const plsvo_match_batch* 
     CK(cudaMemcpyAsync(a.out_A, out->A_cur_ref, n * 4 * sizeof(double), cudaMemcpyHostToDevice, s));
   }
   CK(kernel_timer(c, 0, s));
-  CK(match_direct_kernel_launch(a, s));
+  CK(atan ? match_direct_atan_kernel_launch(a, s) : match_direct_kernel_launch(a, s));
   CK(kernel_timer(c, 1, s));
   c->launches += 1;
   CK(cudaMemcpyAsync(out->px_cur, a.out_px, n * 2 * sizeof(double), cudaMemcpyDeviceToHost, s));
@@ -2553,6 +2565,12 @@ extern "C" int plsvo_track_raw_multicam_batch_run(plsvo_ctx* ctx, const plsvo_ra
 extern "C" int plsvo_match_direct_batch_run(plsvo_ctx* ctx, const plsvo_match_batch* in, const plsvo_match_result* out) {
   if (!ctx || !in || !out) return PLSVO_ERR_INVALID;
   return settled(CTX(ctx), match_direct_batch_run_body(ctx, in, out));
+}
+
+extern "C" int plsvo_match_direct_atan_batch_run(plsvo_ctx* ctx, const plsvo_atan_camera* cam, const plsvo_match_batch* in,
+                                                 const plsvo_match_result* out) {
+  if (!ctx || !cam || !in || !out) return PLSVO_ERR_INVALID;
+  return settled(CTX(ctx), match_direct_batch_run_body(ctx, in, out, cam));
 }
 
 extern "C" int plsvo_structopt_batch_run(plsvo_ctx* ctx, const plsvo_structopt_batch* in, const plsvo_structopt_result* out) {

@@ -13,6 +13,11 @@
 #include "../../include/plsvo_b200.h"
 #include "plsvo_shim.h"
 
+#include <vikit/atan_camera.h>
+// A weak reference, as plsvo_shim.cpp's to the ATAN alignment call: the shim is also linked against implementations of
+// the C ABI that answer only the pinhole calls; there DirectMatcher::run on ATAN frames returns PLSVO_ERR_CUDA.
+#pragma weak plsvo_match_direct_atan_batch_run
+
 namespace plsvo {
 namespace b200 {
 namespace {
@@ -30,6 +35,21 @@ bool camera_of(const Frame& f, plsvo_camera* cam) {
   cam->reserved0 = cam->reserved1 = 0;
   cam->fx = pin->fx(), cam->fy = pin->fy(), cam->cx = pin->cx(), cam->cy = pin->cy();
   return true;
+}
+// The frame's camera for DirectMatcher: the undistorted pinhole (returns 0) or vk::ATANCamera (returns 1; *atan receives the
+// constructor arguments recovered from its members, fx = fx_ / width, cx = (cx_ + 0.5) / width, d0 = s_, as
+// plsvo_shim.cpp's camera_of does, and cam its image size).  -1 for any other model.
+int match_camera_of(const Frame& f, plsvo_camera* cam, plsvo_atan_camera* atan) {
+  if (camera_of(f, cam)) return 0;
+  const vk::ATANCamera* at = dynamic_cast<const vk::ATANCamera*>(f.cam_);
+  if (!at) return -1;
+  const double w = at->width(), h = at->height();
+  std::memset(cam, 0, sizeof *cam);
+  cam->width = at->width(), cam->height = at->height();
+  atan->width = at->width(), atan->height = at->height();
+  atan->fx = at->fx_ / w, atan->fy = at->fy_ / h, atan->cx = (at->cx_ + 0.5) / w, atan->cy = (at->cy_ + 0.5) / h;
+  atan->d0 = at->s_;
+  return 1;
 }
 template <class V>
 void put(std::vector<double>& dst, const V& v, int n) {
@@ -206,7 +226,10 @@ int DirectMatcher::run() {
   }
   plsvo_match_batch b;
   std::memset(&b, 0, sizeof b);
-  if (!camera_of(cur_frame, &b.cam)) return PLSVO_ERR_INVALID;
+  plsvo_atan_camera atan;
+  const int model = match_camera_of(cur_frame, &b.cam, &atan);
+  if (model < 0) return PLSVO_ERR_INVALID;
+  if (model == 1 && !plsvo_match_direct_atan_batch_run) return PLSVO_ERR_CUDA;
   b.n_features = (int32_t)n, b.n_ref_images = (int32_t)ref_frames_.size(), b.n_cur_images = 1;
   b.n_pyr_levels = (int32_t)Config::nPyrLevels(), b.n_iter = align_max_iter_;
   std::vector<double> T_ref(7 * ref_frames_.size()), T_cur(7);
@@ -244,7 +267,7 @@ int DirectMatcher::run() {
       !b.pos || !b.px_cur || !r.px_cur || !r.success || !r.search_level || !r.A_cur_ref)
     return session.fail(PLSVO_ERR_INVALID, "DirectMatcher::run (scratch)");
   std::memset(r.A_cur_ref, 0, 4 * n * sizeof(double));  // rows the kernel leaves untouched come back as sent
-  const int rc = plsvo_match_direct_batch_run(session.ctx(), &b, &r);
+  const int rc = model == 1 ? plsvo_match_direct_atan_batch_run(session.ctx(), &atan, &b, &r) : plsvo_match_direct_batch_run(session.ctx(), &b, &r);
   if (rc != PLSVO_OK) return session.fail(rc, "DirectMatcher::run");
   std::memcpy(px_out_.data(), r.px_cur, 2 * n * sizeof(double));
   std::memcpy(success_.data(), r.success, n);

@@ -35,7 +35,9 @@ namespace b200 {
 ///   0. reset(*frame) at the top of reprojectMap;
 ///   1. enqueue() every candidate after the grids are filled — this runs Point/LineSeg::getCloseViewObs (list logic,
 ///      stays on the host, src/feature3D.cpp:80-124) and records the reference observation;
-///   2. run() — ONE plsvo_match_direct_batch_run for the frame (a segment is two rows);
+///   2. run() — ONE plsvo_match_direct_batch_run for the frame (a segment is two rows), or, when the frame's cam_ is a
+///      vk::ATANCamera, ONE plsvo_match_direct_atan_batch_run with that camera (its constructor arguments rebuilt from
+///      the members fx_..cy_, s_; the keyframes are taken to share it, as in a reference pipeline);
 ///   3. the reference's own cell loops replay unchanged, with matcher_.findMatchDirect(...) replaced by
 ///      findMatchDirect(k, ...), which returns what Matcher::findMatchDirect would have returned for candidate k and
 ///      leaves search_level_ / ref_ftr_ / A_cur_ref_ as the Matcher members would be left (Reprojector::refine reads
@@ -109,7 +111,9 @@ class DepthFilterB200 : public DepthFilter {
  public:
   DepthFilterB200(feature_detection::DetectorPtr<PointFeat> pt_feature_detector, feature_detection::DetectorPtr<LineFeat> seg_feature_detector,
                   callback_t seed_converged_cb, callback_t_ls seed_converged_cb_ls);
-  /// C-ABI status of the last updateSeeds (PLSVO_OK = 0).  On failure the seeds are left as they were.
+  /// C-ABI status of the last updateSeeds (PLSVO_OK = 0).  On failure the seeds are left as they were.  Frames whose
+  /// cam_ is a vk::ATANCamera are not supported (the seed updates have no ATAN path): updateSeeds then sets an error
+  /// status and leaves every seed as it was.
   int last_status() const { return last_status_; }
 
  protected:

@@ -853,10 +853,12 @@ class MatchData:
 
 def make_match_batch(cam: Camera = VGA, n: int = 2000, n_ref: int = 3, n_cur: int = 3, n_pyr_levels: int = 3, seed: int = 7000,
                      device: str | torch.device = "cpu", motion_t: float = 0.08, motion_r: float = 0.04,
-                     edgelet_frac: float = 0.25, noise_px: float = 1.5, scene: Scene | None = None) -> MatchData:
+                     edgelet_frac: float = 0.25, noise_px: float = 1.5, scene: Scene | None = None, atan=None) -> MatchData:
     """n reprojection candidates: a reference observation (keyframe r, pixel, bearing, level), its 3D point on the
     synthetic surface, and the projection into current frame c perturbed by up to `noise_px` (what the reprojector
-    hands to findMatchDirect).  A few candidates sit at the image border / far outside to exercise the early-outs."""
+    hands to findMatchDirect).  A few candidates sit at the image border / far outside to exercise the early-outs.
+    atan: an ATAN (FOV) camera (api.ATANCamera) of cam's size.  Both pyramids are then rendered through it, the bearings
+    are its cam2world and px_cur_gt its world2cam; the random draws are the same as without it."""
     dev = torch.device(device)
     scene = scene or Scene()
     rng = np.random.Generator(np.random.PCG64(seed))
@@ -867,8 +869,8 @@ def make_match_batch(cam: Camera = VGA, n: int = 2000, n_ref: int = 3, n_cur: in
     R_ref, t_ref = se3_exp_Rt(torch.tensor(xi_ref, **f64))
     R_cur, t_cur = se3_exp_Rt(torch.tensor(xi_cur, **f64))
     T_ref_w, T_cur_w = pose7_from_Rt(R_ref, t_ref), pose7_from_Rt(R_cur, t_cur)
-    ref_pyr = {l: np.ascontiguousarray(p.cpu().numpy()) for l, p in enumerate(build_pyramid(scene.render(cam, T_ref_w), n_pyr_levels))}
-    cur_pyr = {l: np.ascontiguousarray(p.cpu().numpy()) for l, p in enumerate(build_pyramid(scene.render(cam, T_cur_w), n_pyr_levels))}
+    ref_pyr = {l: np.ascontiguousarray(p.cpu().numpy()) for l, p in enumerate(build_pyramid(scene.render(cam, T_ref_w, atan=atan), n_pyr_levels))}
+    cur_pyr = {l: np.ascontiguousarray(p.cpu().numpy()) for l, p in enumerate(build_pyramid(scene.render(cam, T_cur_w, atan=atan), n_pyr_levels))}
     ref_index = rng.integers(0, n_ref, n).astype(np.int32)
     cur_index = rng.integers(0, n_cur, n).astype(np.int32)
     ref_level = rng.integers(0, n_pyr_levels, n).astype(np.int32)
@@ -877,13 +879,20 @@ def make_match_batch(cam: Camera = VGA, n: int = 2000, n_ref: int = 3, n_cur: in
     ref_px[:k] = [[3.0, 50.0], [cam.width - 4.0, 50.0], [100.0, 2.0], [100.0, cam.height - 3.0], [6.0 * 4, 6.0 * 4],
                   [cam.width / 2, cam.height / 2], [7.9, 200.0], [cam.width - 7.0, cam.height - 7.0]][:k]
     px_t = torch.tensor(ref_px, **f64)
-    d = torch.stack([(px_t[:, 0] - cam.cx) / cam.fx, (px_t[:, 1] - cam.cy) / cam.fy, torch.ones_like(px_t[:, 0])], -1)
-    ref_f = d / d.norm(dim=-1, keepdim=True)
+    if atan is None:
+        d = torch.stack([(px_t[:, 0] - cam.cx) / cam.fx, (px_t[:, 1] - cam.cy) / cam.fy, torch.ones_like(px_t[:, 0])], -1)
+        ref_f = d / d.norm(dim=-1, keepdim=True)
+    else:
+        d = atan_rays(atan, px_t[:, 0], px_t[:, 1])
+        ref_f = torch.tensor(atan.cam2world(ref_px), **f64)
     ridx = torch.tensor(ref_index, device=dev, dtype=torch.long)
     cidx = torch.tensor(cur_index, device=dev, dtype=torch.long)
     pos = scene.intersect(R_ref[ridx], t_ref[ridx], d[:, None, :])[:, 0, :]
     p_cur = (R_cur[cidx] @ pos[..., None])[..., 0] + t_cur[cidx]
-    px_gt = torch.stack([cam.fx * p_cur[:, 0] / p_cur[:, 2] + cam.cx, cam.fy * p_cur[:, 1] / p_cur[:, 2] + cam.cy], -1).cpu().numpy()
+    if atan is None:
+        px_gt = torch.stack([cam.fx * p_cur[:, 0] / p_cur[:, 2] + cam.cx, cam.fy * p_cur[:, 1] / p_cur[:, 2] + cam.cy], -1).cpu().numpy()
+    else:
+        px_gt = atan.world2cam(p_cur.cpu().numpy())
     px_cur = px_gt + rng.uniform(-noise_px, noise_px, (n, 2))
     is_edgelet = (rng.uniform(size=n) < edgelet_frac).astype(np.uint8)
     ang = rng.uniform(0, 2 * math.pi, n)
