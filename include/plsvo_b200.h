@@ -452,8 +452,9 @@ int plsvo_track_atan_batch_run(plsvo_ctx* ctx, const plsvo_atan_camera* cam, con
  *   variant left, or PLSVO_VARIANT pinned, it returns PLSVO_ERR_INVALID (DESIGN.md §4.11).
  * - Raw frames: plsvo_*_raw_multicam_batch_run above.
  * - ATAN (FOV) cameras per pair: plsvo_*_atan_multicam_batch_run below.
- * - Out of scope: a ragged (unpadded) frame layout, pinhole and ATAN pairs in one batch, the arrival-gated streamed path, separate upload / launch / download legs, dist.align_sharded, the next-row kernels (direct matching,
- *   seed updates, structure optimisation) and the drop-in shim (one frame per call, nothing to batch).
+ * - Out of scope: a ragged (unpadded) frame layout, pinhole and ATAN pairs in one batch, the arrival-gated streamed path, separate upload / launch / download legs, dist.align_sharded, the seed updates
+ *   and the drop-in shim (one frame per call, nothing to batch).  Direct matching with a camera per image:
+ *   plsvo_match_direct_multicam_batch_run.
  * ---------------------------------------------------------------------------------------- */
 int plsvo_align_multicam_batch_run(plsvo_ctx* ctx, const plsvo_camera* cams /* [B] */, const plsvo_align_batch* batch,
                                    const plsvo_align_params* params, const plsvo_align_result* out);
@@ -487,8 +488,8 @@ int plsvo_track_multicam_batch_run(plsvo_ctx* ctx, const plsvo_camera* cams /* [
  *   kernels returns PLSVO_ERR_CUDA.
  * - The kernels keep the pair's members, size and distortion terms in 128 bytes of shared memory per CTA, planned for as
  *   for the multicam kernels (DESIGN.md §4.14).
- * - Out of scope: pinhole and ATAN pairs in one batch, raw frames, the arrival-gated path, a ragged layout, the next-row
- *   kernels and the drop-in shim.
+ * - Out of scope: pinhole and ATAN pairs in one batch, raw frames, the arrival-gated path, a ragged layout, the seed
+ *   updates and the drop-in shim.  Direct matching with a camera per image: plsvo_match_direct_multicam_batch_run.
  * ---------------------------------------------------------------------------------------- */
 int plsvo_align_atan_multicam_batch_run(plsvo_ctx* ctx, const plsvo_atan_camera* cams /* [B] */, const plsvo_align_batch* batch,
                                         const plsvo_align_params* params, const plsvo_align_result* out);
@@ -608,10 +609,50 @@ int plsvo_match_direct_batch_run(plsvo_ctx* ctx, const plsvo_match_batch* in, co
  *   level, success and px_cur are byte for byte what the reference computes from the returned A_cur_ref.  A candidate
  *   whose five projections call neither tan nor atan (d0 == 0, or every argument inside both cut-offs) matches the
  *   reference byte for byte, A_cur_ref included.
- * - Out of scope: the depth-filter seed updates (findEpipolarMatchDirect) for ATAN frames, a camera per image or per
- *   candidate, pinhole and ATAN candidates in one call, raw frames. */
+ * - Out of scope: the depth-filter seed updates (findEpipolarMatchDirect) for ATAN frames, raw frames.  A camera per
+ *   image, pinhole and ATAN candidates in one call: plsvo_match_direct_multicam_batch_run below. */
 int plsvo_match_direct_atan_batch_run(plsvo_ctx* ctx, const plsvo_atan_camera* cam, const plsvo_match_batch* in,
                                       const plsvo_match_result* out);
+
+/* ---- Matcher::findMatchDirect for images from differently calibrated cameras --------------------
+ * plsvo_match_direct_batch_run with a camera per image, pinhole or ATAN, in the padded slots of the multicam calls: one
+ * call serves the keyframes and current frames of many visual-odometry streams.  In the reference the cameras belong to
+ * the frames (ref_ftr_->frame->cam_ and cur_frame.cam_, src/matcher.cpp:168-176), and a candidate may pair a keyframe
+ * and a current frame from different cameras.
+ * - Slot: of in->cam only width and height are used; they are the slot.  Every image sits in a slot-sized frame at the
+ *   batch's pitches and strides.  Ref image r's camera is cams[cam_of_ref[r]], current image c's cams[cam_of_cur[c]];
+ *   the image's pixels are that camera's width x height in the top-left corner, at level l (width >> l) x (height >> l).
+ *   The bytes outside that region (the padding) never reach a result.
+ * - Candidate i reads its ref image's camera for the in-frame test, the warpAffine bounds and cam2world in
+ *   getWarpMatrixAffine; its current image's camera for world2cam in getWarpMatrixAffine and the align2D / align1D bounds
+ *   at the search level.
+ * - A pinhole camera (model PLSVO_CAMERA_PINHOLE) is plsvo_match_batch::cam of plsvo_match_direct_batch_run: size and
+ *   fx..cy in pixels.  An ATAN camera (PLSVO_CAMERA_ATAN) is the constructor's arguments, as for
+ *   plsvo_match_direct_atan_batch_run, and its members are derived exactly as that call derives them.  The other member
+ *   of the record is ignored.
+ * - Exactness: a candidate whose two images share camera k gives byte for byte the outputs of the one-camera call
+ *   (plsvo_match_direct_batch_run or plsvo_match_direct_atan_batch_run with k, the frames cut out of their slots).  A
+ *   candidate with two pinhole cameras matches the reference byte for byte; one with an ATAN camera meets the contract of
+ *   plsvo_match_direct_atan_batch_run.
+ * - NULL cams, cam_of_ref or cam_of_cur; n_cams < 1; an index outside [0, n_cams); an unknown model; a pinhole camera
+ *   with a non-finite fx, fy, cx or cy or with fx or fy equal to 0; an ATAN camera plsvo_match_direct_atan_batch_run
+ *   rejects; a camera wider or taller than the slot; or a camera used at a level below one pixel (a ref image's at its
+ *   candidates' ref_level, a current image's at n_pyr_levels - 1) returns PLSVO_ERR_INVALID, with the index in the
+ *   message, before anything is queued; the context stays usable.  A library built without the kernel returns
+ *   PLSVO_ERR_CUDA.
+ * - Out of scope: the depth-filter seed updates per camera, raw frames, a ragged frame layout, a camera per candidate. */
+#define PLSVO_CAMERA_PINHOLE 0
+#define PLSVO_CAMERA_ATAN 1
+typedef struct plsvo_match_camera {
+  int32_t model, reserved;
+  plsvo_camera pinhole;   /* model PINHOLE: size and fx..cy in pixels, as plsvo_match_batch::cam */
+  plsvo_atan_camera atan; /* model ATAN: the constructor's arguments, as for plsvo_match_direct_atan_batch_run */
+} plsvo_match_camera;
+
+int plsvo_match_direct_multicam_batch_run(plsvo_ctx* ctx, const plsvo_match_camera* cams, int32_t n_cams,
+                                          const int32_t* cam_of_ref /* [n_ref_images] */,
+                                          const int32_t* cam_of_cur /* [n_cur_images] */, const plsvo_match_batch* in,
+                                          const plsvo_match_result* out);
 
 /* ---- Structure optimisation: Point::optimize / LineSeg::optimize (SURVEY.md §8f rank 3, "next") ---
  * Replaces, for a batch of 3D features, include/plsvo/feature3D.h:120,157 / src/feature3D_impl.cpp:36-95,

@@ -180,6 +180,27 @@ class AtanCamera(C.Structure):
                 ("cy", C.c_double), ("d0", C.c_double)]
 
 
+CAMERA_PINHOLE, CAMERA_ATAN = 0, 1  # PLSVO_CAMERA_PINHOLE, PLSVO_CAMERA_ATAN
+
+
+class MatchCamera(C.Structure):
+    """plsvo_match_camera: one camera of plsvo_match_direct_multicam_batch_run, a pinhole (size and fx..cy in pixels, as
+    plsvo_match_batch::cam) or an ATAN camera (its constructor arguments), chosen by `model`."""
+    _fields_ = [("model", C.c_int32), ("reserved", C.c_int32), ("pinhole", Camera), ("atan", AtanCamera)]
+
+
+def make_match_cameras(cameras):
+    """plsvo_match_camera[K] from a sequence of api.ATANCamera / synth.Camera (undistorted pinhole) objects."""
+    arr = (MatchCamera * len(cameras))()
+    for k, cam in enumerate(cameras):
+        if hasattr(cam, "struct") and isinstance(cam.struct, AtanCamera):
+            arr[k].model, arr[k].atan = CAMERA_ATAN, cam.struct
+        else:
+            arr[k].model = CAMERA_PINHOLE
+            arr[k].pinhole = Camera(cam.width, cam.height, 0, 0, cam.fx, cam.fy, cam.cx, cam.cy)
+    return arr
+
+
 def make_cameras(cameras, cam, batch: int, sizes=None):
     """plsvo_camera[B] of a multicam call from `cameras`, an array-like [B, 4] of (fx, fy, cx, cy) rows.  Each has the
     image size of `cam` (the batch's camera, whose size is the slot every pair's frames sit in), or with `sizes`, an
@@ -550,6 +571,8 @@ ABI_SYMBOLS = [
     ("plsvo_align1d_batch_run", C.c_int, [C.c_void_p, _P(Align1DBatch), _P(Align1DResult)]),
     ("plsvo_match_direct_batch_run", C.c_int, [C.c_void_p, _P(MatchBatch), _P(MatchResult)]),
     ("plsvo_match_direct_atan_batch_run", C.c_int, [C.c_void_p, _P(AtanCamera), _P(MatchBatch), _P(MatchResult)]),
+    ("plsvo_match_direct_multicam_batch_run", C.c_int, [C.c_void_p, _P(MatchCamera), C.c_int32, _P(C.c_int32), _P(C.c_int32),
+                                                        _P(MatchBatch), _P(MatchResult)]),
     ("plsvo_seed_update_batch_run", C.c_int, [C.c_void_p, _P(SeedBatch), _P(SeedResult)]),
     ("plsvo_line_seed_update_batch_run", C.c_int, [C.c_void_p, _P(LineSeedBatch), _P(LineSeedResult)]),
     ("plsvo_structopt_batch_run", C.c_int, [C.c_void_p, _P(StructOptBatch), _P(StructOptResult)]),

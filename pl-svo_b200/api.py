@@ -539,24 +539,58 @@ class Matcher:
         self.align_max_iter = align_max_iter  # Matcher::Options::align_max_iter
         self.ctx = ctx or default_context()
 
-    def findMatchDirect(self, data, camera: "ATANCamera | None" = None) -> abi.MatchOut:
+    def findMatchDirect(self, data, camera: "ATANCamera | list | None" = None, cam_of_ref=None, cam_of_cur=None) -> abi.MatchOut:
         """data: synth.MatchData-like batch -> px_cur (refined, level-0 pixels), success flags, search levels.
         camera: an ATANCamera when the keyframes and current frames come from one (plsvo_match_direct_atan_batch_run;
-        data.cam then only gives the image size); None for the undistorted pinhole of data.cam."""
+        data.cam then only gives the image size); None for the undistorted pinhole of data.cam.  Or a sequence of cameras,
+        each an ATANCamera or an undistorted pinhole given as a synth.Camera, with cam_of_ref [n_ref_images] and
+        cam_of_cur [n_cur_images] indexing it: every image is seen through its own camera
+        (plsvo_match_direct_multicam_batch_run; data.cam then only gives the slot size, synth.make_match_multicam_batch)."""
         data.n_iter = self.align_max_iter
-        if camera is not None:
+        multi = _match_cameras_arg(camera, cam_of_ref, cam_of_cur, data)
+        if camera is not None and multi is None:
             if not isinstance(camera, ATANCamera):
                 raise TypeError(f"findMatchDirect: camera must be an ATANCamera or None, not {type(camera).__name__}")
             camera._check(data)
         b, keep = abi.make_match_batch(data)
         out = abi.MatchOut(data.n)
-        if camera is not None:
+        if multi is not None:
+            cams, ref, cur = multi
+            self.ctx.check(self.ctx.lib.plsvo_match_direct_multicam_batch_run(
+                self.ctx.handle, cams, len(cams), ref.ctypes.data_as(C.POINTER(C.c_int32)), cur.ctypes.data_as(C.POINTER(C.c_int32)),
+                C.byref(b), C.byref(out.struct)), "plsvo_match_direct_multicam_batch_run")
+        elif camera is not None:
             self.ctx.check(self.ctx.lib.plsvo_match_direct_atan_batch_run(self.ctx.handle, C.byref(camera.struct), C.byref(b),
                                                                           C.byref(out.struct)), "plsvo_match_direct_atan_batch_run")
         else:
             self.ctx.check(self.ctx.lib.plsvo_match_direct_batch_run(self.ctx.handle, C.byref(b), C.byref(out.struct)),
                            "plsvo_match_direct_batch_run")
         return out
+
+
+def _match_cameras_arg(camera, cam_of_ref, cam_of_cur, data):
+    """(plsvo_match_camera[K], cam_of_ref, cam_of_cur as int32 arrays) of the per-image match call when `camera` is a
+    sequence; None for one camera or none.  Mismatched arguments raise PlsvoError; the values (index ranges, camera sizes
+    and parameters) are the C ABI's to check."""
+    import numpy as np
+
+    seq = isinstance(camera, (list, tuple))
+    if not seq:
+        if cam_of_ref is not None or cam_of_cur is not None:
+            raise PlsvoError("cam_of_ref= and cam_of_cur= select cameras per image: camera must then be a sequence of cameras")
+        return None
+    if cam_of_ref is None or cam_of_cur is None:
+        raise PlsvoError("camera= as a sequence needs cam_of_ref= and cam_of_cur=")
+    if len(camera) == 0:
+        raise PlsvoError("camera= is an empty sequence")
+    for k, c in enumerate(camera):
+        if not isinstance(c, ATANCamera) and not all(hasattr(c, f) for f in ("width", "height", "fx", "fy", "cx", "cy")):
+            raise PlsvoError(f"camera[{k}] must be an ATANCamera or a synth.Camera, not {type(c).__name__}")
+    ref, cur = (np.ascontiguousarray(x) for x in (cam_of_ref, cam_of_cur))
+    for name, x, n in (("cam_of_ref", ref, data.T_ref_w.shape[0]), ("cam_of_cur", cur, data.T_cur_w.shape[0])):
+        if x.shape != (n,) or not np.issubdtype(x.dtype, np.integer):
+            raise PlsvoError(f"{name} must be integers of shape [{n}] (a camera per image), got {x.dtype} {list(x.shape)}")
+    return abi.make_match_cameras(camera), ref.astype(np.int32), cur.astype(np.int32)
 
 
 def optimizeStructure(data, ctx: Context | None = None) -> abi.StructOptOut:

@@ -240,6 +240,14 @@ cudaError_t align2d_kernel_launch(const Align2DArgs& a, cudaStream_t s);
 cudaError_t align1d_kernel_launch(const Align2DArgs& a, cudaStream_t s);
 
 // ---------------------------------------------------------------------------------------------
+// One camera of the per-image kernel, as the host derives it from a plsvo_match_camera: the pinhole's fx..cy, or the
+// vk::ATANCamera members fx_..cy_ and distortion terms s_, s_inv_, tans_, tans_inv_ (zero for a pinhole).
+struct MatchCamRecord {
+  double fx, fy, cx, cy;
+  int32_t width, height;
+  int32_t model, reserved;  // PLSVO_CAMERA_PINHOLE or PLSVO_CAMERA_ATAN
+  double s, s_inv, tans, tans_inv;
+};
 struct MatchArgs {
   int n, n_iter, n_pyr_levels, width, height;
   double fx, fy, cx, cy;
@@ -267,11 +275,18 @@ struct MatchArgs {
   // vk::ATANCamera distortion (read by the ATAN kernel only; fx, fy, cx, cy above then hold fx_, fy_, cx_, cy_):
   // s_ = d0, s_inv_ = 1/s_, tans_ = 2 tan(s_/2), tans_inv_ = 1/tans_, all zero when s_ == 0
   double atan_s, atan_s_inv, atan_tans, atan_tans_inv;
+  // A camera per image (the per-image kernel only; width / height above are then the slot): image r of the keyframes
+  // is seen through cams[cam_of_ref[r]], image c of the current frames through cams[cam_of_cur[c]]
+  const MatchCamRecord* cams;  // device, [n_cams]
+  const int32_t* cam_of_ref;          // device, [n_ref_images]
+  const int32_t* cam_of_cur;          // device, [n_cur_images]
 };
 cudaError_t match_direct_kernel_launch(const MatchArgs& a, cudaStream_t s);
 // The same kernel with the vk::ATANCamera warp matrix (plsvo_match_direct_atan_batch_run).  Weak, as the ATAN alignment
 // launchers: the host-pipeline model of the tests need not provide it, and the ATAN entry point then reports it missing.
 __attribute__((weak)) cudaError_t match_direct_atan_kernel_launch(const MatchArgs& a, cudaStream_t s);
+// The same kernel with a camera per image (plsvo_match_direct_multicam_batch_run).  Weak, for the same reason.
+__attribute__((weak)) cudaError_t match_direct_multicam_kernel_launch(const MatchArgs& a, cudaStream_t s);
 
 // ---------------------------------------------------------------------------------------------
 struct SeedArgs {

@@ -89,7 +89,8 @@ struct plsvo_ctx_impl {
   DevBuf y_img;  // pyramid levels
   DevBuf f_img, f_idx, f_lvl, f_border, f_ref, f_px, f_opx, f_oconv, f_dir, f_ohinv;  // align2D / align1D
   DevBuf m_ref_img, m_cur_img, m_T_ref, m_T_cur, m_ridx, m_cidx, m_px, m_f, m_lvl, m_edge, m_grad, m_pos, m_pxc, m_opx, m_osucc,
-      m_olvl, m_oA;  // findMatchDirect
+      m_olvl, m_oA, m_cams, m_cam_of_ref, m_cam_of_cur;  // findMatchDirect
+  std::vector<MatchCamRecord> h_match_cams;  // the camera records of a per-image match call, staged for the upload
   DevBuf d_sa, d_sb, d_smu, d_szr, d_ssig, d_smu_e, d_szr_e, d_ssig_e, d_sout;  // depth-filter seeds
   DevBuf s_T, s_pb, s_pf, s_pof, s_pp, s_sb, s_sf, s_ssf, s_sef, s_sp, s_ep, s_out;  // structure optimisation
   // undistortion: raw frames, and the map of the camera in u_cam (valid when u_map_ok), built on the device
@@ -1819,10 +1820,88 @@ int stage_pyramid(plsvo_ctx_impl* c, DevBuf& buf, const uint8_t* const* img, con
 }
 }  // namespace
 
+namespace {
+
+// The cameras of plsvo_match_direct_multicam_batch_run: cams[n_cams], and the camera of every ref and current image
+struct MatchCameraTable {
+  const plsvo_match_camera* cams;
+  int32_t n_cams;
+  const int32_t* cam_of_ref;
+  const int32_t* cam_of_cur;
+};
+
+// Validates the camera table against the batch (whose description has been checked) and derives into c->h_match_cams one
+// record per camera: a pinhole's fx..cy as given, an ATAN camera's members and distortion terms by atan_members, as the
+// one-camera calls derive them.  The ref images' cameras at their candidates' levels are checked with the candidates.
+// Nothing is queued here.
+int match_camera_table(plsvo_ctx_impl* c, const MatchCameraTable& t, const plsvo_match_batch* in) {
+  if (!t.cams || !t.cam_of_ref || !t.cam_of_cur) return fail(c, PLSVO_ERR_INVALID, "cams, cam_of_ref or cam_of_cur is NULL");
+  if (t.n_cams < 1) return fail(c, PLSVO_ERR_INVALID, "n_cams must be at least 1");
+  char msg[224];
+  c->h_match_cams.assign((size_t)t.n_cams, MatchCamRecord{});
+  for (int k = 0; k < t.n_cams; ++k) {
+    const plsvo_match_camera& m = t.cams[k];
+    MatchCamRecord& r = c->h_match_cams[k];
+    r.model = m.model;
+    if (m.model == PLSVO_CAMERA_PINHOLE) {
+      const plsvo_camera& p = m.pinhole;
+      if (!std::isfinite(p.fx) || !std::isfinite(p.fy) || !std::isfinite(p.cx) || !std::isfinite(p.cy)) {
+        snprintf(msg, sizeof msg, "cams[%d] has a non-finite fx, fy, cx or cy", k);
+        return fail(c, PLSVO_ERR_INVALID, msg);
+      }
+      if (p.fx == 0.0 || p.fy == 0.0) {
+        snprintf(msg, sizeof msg, "cams[%d].fx and fy must be non-zero", k);
+        return fail(c, PLSVO_ERR_INVALID, msg);
+      }
+      r.fx = p.fx, r.fy = p.fy, r.cx = p.cx, r.cy = p.cy, r.width = p.width, r.height = p.height;
+    } else if (m.model == PLSVO_CAMERA_ATAN) {
+      plsvo_camera k_;
+      double terms[4];
+      if (const char* why = atan_members(m.atan, &k_, terms)) {
+        snprintf(msg, sizeof msg, "cams[%d] (ATAN) %s", k, why);
+        return fail(c, PLSVO_ERR_INVALID, msg);
+      }
+      r.fx = k_.fx, r.fy = k_.fy, r.cx = k_.cx, r.cy = k_.cy, r.width = k_.width, r.height = k_.height;
+      r.s = terms[0], r.s_inv = terms[1], r.tans = terms[2], r.tans_inv = terms[3];
+    } else {
+      snprintf(msg, sizeof msg, "cams[%d].model %d is neither PLSVO_CAMERA_PINHOLE nor PLSVO_CAMERA_ATAN", k, m.model);
+      return fail(c, PLSVO_ERR_INVALID, msg);
+    }
+    if (!(r.width >= 1 && r.height >= 1 && r.width <= in->cam.width && r.height <= in->cam.height)) {
+      snprintf(msg, sizeof msg, "cams[%d] is %dx%d, in->cam is %dx%d: every camera must fit inside the batch's image slot", k, r.width,
+               r.height, in->cam.width, in->cam.height);
+      return fail(c, PLSVO_ERR_INVALID, msg);
+    }
+  }
+  for (int i = 0; i < in->n_ref_images; ++i)
+    if (t.cam_of_ref[i] < 0 || t.cam_of_ref[i] >= t.n_cams) {
+      snprintf(msg, sizeof msg, "cam_of_ref[%d] = %d is outside [0, %d)", i, t.cam_of_ref[i], t.n_cams);
+      return fail(c, PLSVO_ERR_INVALID, msg);
+    }
+  const int top = in->n_pyr_levels - 1;  // the deepest level align2D / align1D may search
+  for (int i = 0; i < in->n_cur_images; ++i) {
+    const int k = t.cam_of_cur[i];
+    if (k < 0 || k >= t.n_cams) {
+      snprintf(msg, sizeof msg, "cam_of_cur[%d] = %d is outside [0, %d)", i, k, t.n_cams);
+      return fail(c, PLSVO_ERR_INVALID, msg);
+    }
+    if ((c->h_match_cams[k].width >> top) <= 0 || (c->h_match_cams[k].height >> top) <= 0) {
+      snprintf(msg, sizeof msg, "cams[%d] (current image %d) is %dx%d: pyramid level %d smaller than one pixel", k, i,
+               c->h_match_cams[k].width, c->h_match_cams[k].height, top);
+      return fail(c, PLSVO_ERR_INVALID, msg);
+    }
+  }
+  if (!match_direct_multicam_kernel_launch) return fail(c, PLSVO_ERR_CUDA, "this library was built without the per-image matching kernel");
+  return PLSVO_OK;
+}
+
+}  // namespace
+
 // atan: NULL for the undistorted pinhole of in->cam, or the vk::ATANCamera both frames are seen through
-// (plsvo_match_direct_atan_batch_run); it is validated, and the kernel's presence checked, before anything is queued.
+// (plsvo_match_direct_atan_batch_run).  multi: NULL, or a camera per image (plsvo_match_direct_multicam_batch_run; in->cam
+// is then the slot).  Either is validated, and the kernel's presence checked, before anything is queued.
 static int match_direct_batch_run_body(plsvo_ctx* ctx, const plsvo_match_batch* in, const plsvo_match_result* out,
-                                       const plsvo_atan_camera* atan = nullptr) {
+                                       const plsvo_atan_camera* atan = nullptr, const MatchCameraTable* multi = nullptr) {
   plsvo_ctx_impl* c = CTX(ctx);
   plsvo_camera k = in->cam;
   double terms[4] = {0.0, 0.0, 0.0, 0.0};
@@ -1835,6 +1914,10 @@ static int match_direct_batch_run_body(plsvo_ctx* ctx, const plsvo_match_batch* 
   if (in->n_features < 0 || in->n_ref_images <= 0 || in->n_cur_images <= 0 || in->cam.width <= 0 || in->cam.height <= 0 ||
       in->n_iter < 0 || in->n_pyr_levels < 1 || in->n_pyr_levels > PLSVO_MAX_LEVELS)
     return fail(c, PLSVO_ERR_INVALID, "match batch description");
+  if (multi) {
+    const int rc = match_camera_table(c, *multi, in);
+    if (rc != PLSVO_OK) return rc;
+  }
   if (in->n_features == 0) return PLSVO_OK;
   if (!in->T_ref_w || !in->T_cur_w || !in->ref_index || !in->cur_index || !in->ref_px || !in->ref_f || !in->ref_level || !in->pos ||
       !in->px_cur || !out->px_cur || !out->success)
@@ -1848,6 +1931,15 @@ static int match_direct_batch_run_body(plsvo_ctx* ctx, const plsvo_match_batch* 
     if (l < 0 || l >= PLSVO_MAX_LEVELS || !in->ref_img[l] || in->ref_index[i] < 0 || in->ref_index[i] >= in->n_ref_images ||
         in->cur_index[i] < 0 || in->cur_index[i] >= in->n_cur_images)
       return fail(c, PLSVO_ERR_INVALID, "match candidate refers to a missing level or frame");
+    if (multi) {  // the ref image's camera at the candidate's level
+      const MatchCamRecord& m = c->h_match_cams[multi->cam_of_ref[in->ref_index[i]]];
+      if ((m.width >> l) <= 0 || (m.height >> l) <= 0) {
+        char msg[224];
+        snprintf(msg, sizeof msg, "cams[%d] (ref image %d, candidate %zu) is %dx%d: pyramid level %d smaller than one pixel",
+                 multi->cam_of_ref[in->ref_index[i]], in->ref_index[i], i, m.width, m.height, l);
+        return fail(c, PLSVO_ERR_INVALID, msg);
+      }
+    }
   }
   CK(cudaSetDevice(c->device));
   cudaStream_t s = c->stream;
@@ -1874,6 +1966,11 @@ static int match_direct_batch_run_body(plsvo_ctx* ctx, const plsvo_match_batch* 
   CK(up(c->m_grad, in->is_edgelet ? in->ref_grad : nullptr, n * 2, s, &a.ref_grad));
   CK(up(c->m_pos, in->pos, n * 3, s, &a.pos));
   CK(up(c->m_pxc, in->px_cur, n * 2, s, &a.px_cur));
+  if (multi) {
+    CK(up(c->m_cams, c->h_match_cams.data(), c->h_match_cams.size(), s, &a.cams));
+    CK(up(c->m_cam_of_ref, multi->cam_of_ref, (size_t)in->n_ref_images, s, &a.cam_of_ref));
+    CK(up(c->m_cam_of_cur, multi->cam_of_cur, (size_t)in->n_cur_images, s, &a.cam_of_cur));
+  }
   CK(ensure(c->m_opx, n * 2 * sizeof(double)));
   CK(ensure(c->m_osucc, n));
   CK(ensure(c->m_olvl, n * sizeof(int32_t)));
@@ -1887,7 +1984,7 @@ static int match_direct_batch_run_body(plsvo_ctx* ctx, const plsvo_match_batch* 
     CK(cudaMemcpyAsync(a.out_A, out->A_cur_ref, n * 4 * sizeof(double), cudaMemcpyHostToDevice, s));
   }
   CK(kernel_timer(c, 0, s));
-  CK(atan ? match_direct_atan_kernel_launch(a, s) : match_direct_kernel_launch(a, s));
+  CK(multi ? match_direct_multicam_kernel_launch(a, s) : atan ? match_direct_atan_kernel_launch(a, s) : match_direct_kernel_launch(a, s));
   CK(kernel_timer(c, 1, s));
   c->launches += 1;
   CK(cudaMemcpyAsync(out->px_cur, a.out_px, n * 2 * sizeof(double), cudaMemcpyDeviceToHost, s));
@@ -2571,6 +2668,14 @@ extern "C" int plsvo_match_direct_atan_batch_run(plsvo_ctx* ctx, const plsvo_ata
                                                  const plsvo_match_result* out) {
   if (!ctx || !cam || !in || !out) return PLSVO_ERR_INVALID;
   return settled(CTX(ctx), match_direct_batch_run_body(ctx, in, out, cam));
+}
+
+extern "C" int plsvo_match_direct_multicam_batch_run(plsvo_ctx* ctx, const plsvo_match_camera* cams, int32_t n_cams,
+                                                     const int32_t* cam_of_ref, const int32_t* cam_of_cur,
+                                                     const plsvo_match_batch* in, const plsvo_match_result* out) {
+  if (!ctx || !in || !out) return PLSVO_ERR_INVALID;
+  const MatchCameraTable t{cams, n_cams, cam_of_ref, cam_of_cur};
+  return settled(CTX(ctx), match_direct_batch_run_body(ctx, in, out, nullptr, &t));
 }
 
 extern "C" int plsvo_structopt_batch_run(plsvo_ctx* ctx, const plsvo_structopt_batch* in, const plsvo_structopt_result* out) {

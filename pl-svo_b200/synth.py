@@ -904,6 +904,124 @@ def make_match_batch(cam: Camera = VGA, n: int = 2000, n_ref: int = 3, n_cur: in
                      pos=c(pos, np.float64), px_cur=c(px_cur, np.float64), px_cur_gt=c(px_gt, np.float64))
 
 
+def make_match_multicam_batch(cams, cam_of_ref, cam_of_cur, n: int = 2000, n_pyr_levels: int = 3, seed: int = 7100,
+                              device: str | torch.device = "cpu", slot: Camera | None = None, fill=0, same_camera_frac: float = 0.5,
+                              motion_t: float = 0.08, motion_r: float = 0.04, edgelet_frac: float = 0.25, noise_px: float = 1.5,
+                              scene: Scene | None = None):
+    """n reprojection candidates over keyframes and current frames from several cameras, the batch of
+    plsvo_match_direct_multicam_batch_run.  cams: undistorted pinholes (Camera) or ATAN cameras (api.ATANCamera), of any
+    sizes; ref image r is seen through cams[cam_of_ref[r]] and current image c through cams[cam_of_cur[c]].  Every image
+    is rendered through its own camera at that camera's size and padded into a slot of `slot`'s size (default: the largest
+    width and height), in the top-left corner, as merge_sizes pads; the padding is `fill`, a byte or a numpy Generator
+    for random bytes.  Each reference pixel lies inside its ref camera's size (the first few on its borders), its bearing is
+    that camera's cam2world and px_cur_gt the current camera's world2cam.  A share `same_camera_frac` of the candidates
+    picks a current image of its keyframe's camera where one exists; the others pick any, so many pair two cameras.
+    Returns (MatchData with cam = slot, parts, groups): for camera k, groups[k] are the positions of the candidates whose
+    two images are both seen through cams[k], and parts[k] their one-camera MatchData, its images cut out of the slots
+    at k's own size (None when groups[k] is empty)."""
+    dev = torch.device(device)
+    scene = scene or Scene()
+    rng = np.random.Generator(np.random.PCG64(seed))
+    f64 = dict(dtype=torch.float64, device=dev)
+    cam_of_ref, cam_of_cur = np.asarray(cam_of_ref, np.int32), np.asarray(cam_of_cur, np.int32)
+    n_ref, n_cur = len(cam_of_ref), len(cam_of_cur)
+    is_atan = [hasattr(c, "s_") for c in cams]
+    size = [Camera(c.width, c.height, 1.0, 1.0, 0.0, 0.0) for c in cams]
+    if slot is None:
+        slot = Camera(max(c.width for c in cams), max(c.height for c in cams), 1.0, 1.0, 0.0, 0.0)
+    if any(c.width > slot.width or c.height > slot.height for c in cams):
+        raise ValueError("every camera must fit inside the slot")
+    xi_ref = np.concatenate([rng.uniform(-0.2, 0.2, (n_ref, 3)), rng.uniform(-0.03, 0.03, (n_ref, 3))], -1)
+    xi_cur = np.concatenate([rng.uniform(-0.2 - motion_t, 0.2 + motion_t, (n_cur, 3)), rng.uniform(-motion_r, motion_r, (n_cur, 3))], -1)
+    xi_cur[:, 2] = rng.uniform(-0.05, 0.45, n_cur)
+    R_ref, t_ref = se3_exp_Rt(torch.tensor(xi_ref, **f64))
+    R_cur, t_cur = se3_exp_Rt(torch.tensor(xi_cur, **f64))
+    T_ref_w, T_cur_w = pose7_from_Rt(R_ref, t_ref), pose7_from_Rt(R_cur, t_cur)
+
+    def pyramids(T, cam_of):
+        pyr = {l: (fill.integers(0, 256, (len(cam_of), slot.height >> l, slot.width >> l), dtype=np.uint8)
+                   if isinstance(fill, np.random.Generator) else np.full((len(cam_of), slot.height >> l, slot.width >> l), fill, np.uint8))
+               for l in range(n_pyr_levels)}
+        for k in np.unique(cam_of):
+            idx = np.flatnonzero(cam_of == k)
+            img = scene.render(cams[k] if not is_atan[k] else size[k], T[torch.as_tensor(idx, device=dev)],
+                               atan=cams[k] if is_atan[k] else None)
+            for l, p in enumerate(build_pyramid(img, n_pyr_levels)):
+                pyr[l][idx, : p.shape[1], : p.shape[2]] = p.cpu().numpy()
+        return pyr
+
+    ref_pyr, cur_pyr = pyramids(T_ref_w, cam_of_ref), pyramids(T_cur_w, cam_of_cur)
+    ref_index = rng.integers(0, n_ref, n).astype(np.int32)
+    cur_index = rng.integers(0, n_cur, n).astype(np.int32)
+    same = rng.uniform(size=n) < same_camera_frac
+    for i in np.flatnonzero(same):
+        mine = np.flatnonzero(cam_of_cur == cam_of_ref[ref_index[i]])
+        if len(mine):
+            cur_index[i] = mine[rng.integers(0, len(mine))]
+    ref_level = rng.integers(0, n_pyr_levels, n).astype(np.int32)
+    kr, kc = cam_of_ref[ref_index], cam_of_cur[cur_index]
+    W = np.array([c.width for c in cams], np.float64)
+    H = np.array([c.height for c in cams], np.float64)
+    ref_px = np.stack([rng.uniform(20, W[kr] - 20), rng.uniform(20, H[kr] - 20)], -1)
+    k = min(8, n)  # the borders of the ref camera, as make_match_batch places them in its one camera
+    w, h = W[kr[:8]], H[kr[:8]]
+    if k == 8:
+        ref_px[:8] = np.stack([[3.0, w[1] - 4.0, 100.0, 100.0, 24.0, w[5] / 2, 7.9, w[7] - 7.0],
+                               [50.0, 50.0, 2.0, h[3] - 3.0, 24.0, h[5] / 2, 200.0, h[7] - 7.0]], -1)
+    d = torch.empty(n, 3, **f64)
+    ref_f = np.empty((n, 3))
+    for kk in np.unique(kr):
+        sel = np.flatnonzero(kr == kk)
+        c = cams[kk]
+        px_t = torch.tensor(ref_px[sel], **f64)
+        if is_atan[kk]:
+            d[sel] = atan_rays(c, px_t[:, 0], px_t[:, 1])
+            ref_f[sel] = c.cam2world(ref_px[sel])
+        else:
+            dd = torch.stack([(px_t[:, 0] - c.cx) / c.fx, (px_t[:, 1] - c.cy) / c.fy, torch.ones_like(px_t[:, 0])], -1)
+            d[sel] = dd
+            ref_f[sel] = (dd / dd.norm(dim=-1, keepdim=True)).cpu().numpy()
+    ridx = torch.tensor(ref_index, device=dev, dtype=torch.long)
+    cidx = torch.tensor(cur_index, device=dev, dtype=torch.long)
+    pos = scene.intersect(R_ref[ridx], t_ref[ridx], d[:, None, :])[:, 0, :]
+    p_cur = ((R_cur[cidx] @ pos[..., None])[..., 0] + t_cur[cidx]).cpu().numpy()
+    px_gt = np.empty((n, 2))
+    for kk in np.unique(kc):
+        sel = np.flatnonzero(kc == kk)
+        c = cams[kk]
+        if is_atan[kk]:
+            px_gt[sel] = c.world2cam(p_cur[sel])
+        else:
+            px_gt[sel] = np.stack([c.fx * p_cur[sel, 0] / p_cur[sel, 2] + c.cx, c.fy * p_cur[sel, 1] / p_cur[sel, 2] + c.cy], -1)
+    px_cur = px_gt + rng.uniform(-noise_px, noise_px, (n, 2))
+    is_edgelet = (rng.uniform(size=n) < edgelet_frac).astype(np.uint8)
+    ang = rng.uniform(0, 2 * math.pi, n)
+    ref_grad = np.stack([np.cos(ang), np.sin(ang)], -1)
+    c64 = lambda a: np.ascontiguousarray(a.cpu().numpy() if isinstance(a, torch.Tensor) else a, dtype=np.float64)  # noqa: E731
+    data = MatchData(cam=slot, n_pyr_levels=n_pyr_levels, ref_pyr=ref_pyr, cur_pyr=cur_pyr, T_ref_w=c64(T_ref_w), T_cur_w=c64(T_cur_w),
+                     ref_index=ref_index, cur_index=cur_index, ref_px=c64(ref_px), ref_f=c64(ref_f), ref_level=ref_level,
+                     is_edgelet=is_edgelet, ref_grad=c64(ref_grad), pos=c64(pos), px_cur=c64(px_cur), px_cur_gt=c64(px_gt))
+    groups, parts = [], []
+    for kk, c in enumerate(cams):
+        g = np.flatnonzero((kr == kk) & (kc == kk))
+        groups.append(g)
+        if not len(g):
+            parts.append(None)
+            continue
+        refs, curs = np.flatnonzero(cam_of_ref == kk), np.flatnonzero(cam_of_cur == kk)
+        rmap, cmap = np.full(n_ref, -1, np.int32), np.full(n_cur, -1, np.int32)
+        rmap[refs], cmap[curs] = np.arange(len(refs)), np.arange(len(curs))
+        one = c if not is_atan[kk] else Camera(c.width, c.height, c.fx_, c.fy_, c.cx_, c.cy_)
+        parts.append(MatchData(cam=one, n_pyr_levels=n_pyr_levels,
+                               ref_pyr={l: im[refs][:, : c.height >> l, : c.width >> l] for l, im in ref_pyr.items()},
+                               cur_pyr={l: im[curs][:, : c.height >> l, : c.width >> l] for l, im in cur_pyr.items()},
+                               T_ref_w=data.T_ref_w[refs], T_cur_w=data.T_cur_w[curs], ref_index=rmap[ref_index[g]],
+                               cur_index=cmap[cur_index[g]], ref_px=data.ref_px[g], ref_f=data.ref_f[g], ref_level=ref_level[g],
+                               is_edgelet=is_edgelet[g], ref_grad=data.ref_grad[g], pos=data.pos[g], px_cur=data.px_cur[g],
+                               px_cur_gt=data.px_cur_gt[g]))
+    return data, parts, groups
+
+
 # ---- structure optimisation: Point::optimize / LineSeg::optimize (SURVEY §8f rank 3) -------------------
 @dataclass
 class StructOptData:
