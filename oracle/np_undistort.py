@@ -14,9 +14,30 @@ def undistort_is_copy(d0) -> bool:
     return not abs(float(d0)) > 1e-7
 
 
+def cv_round(t):
+    """cvRound: round half to even; out of int range (or NaN) gives INT_MIN like cvtsd2si.  int64 array."""
+    r = np.rint(t)
+    ok = (r >= -2147483648.0) & (r <= 2147483647.0)
+    return np.where(ok, np.where(ok, r, 0).astype(np.int64), -2147483648).astype(np.int64)
+
+
+def map_of_rounded(iu, iv):
+    """The CV_16SC2 map from cvRound(u * 32), cvRound(v * 32) as OpenCV's scalar loop stores it: map1 = the (short) casts
+    of iu >> 5, iv >> 5 (wrapping), map2 = (iv & 31) * 32 + (iu & 31)."""
+    map1 = np.stack([(iu >> 5).astype(np.int16), (iv >> 5).astype(np.int16)], -1)  # (short) cast: wraps like C
+    map2 = ((iv & 31) * 32 + (iu & 31)).astype(np.uint16)
+    return map1, map2
+
+
 def undistort_map(width, height, fx, fy, cx, cy, d0=0.0, d1=0.0, d2=0.0, d3=0.0, d4=0.0):
     """cv::initUndistortRectifyMap(cvK_, cvD_, I, cvK_, size, CV_16SC2) -> (map1 int16 [H,W,2], map2 uint16 [H,W]).
     cvK_ / cvD_ are Mat_<float>: every parameter is rounded to float first."""
+    u32, v32 = undistort_coords(width, height, fx, fy, cx, cy, d0, d1, d2, d3, d4)
+    return map_of_rounded(cv_round(u32), cv_round(v32))
+
+
+def undistort_coords(width, height, fx, fy, cx, cy, d0=0.0, d1=0.0, d2=0.0, d3=0.0, d4=0.0):
+    """u * 32 and v * 32 (float64 [H,W]) of every map entry, the values cvRound rounds."""
     fx, fy, cx, cy, k1, k2, p1, p2, k3 = (float(np.float32(v)) for v in (fx, fy, cx, cy, d0, d1, d2, d3, d4))
     # iR = (K R).inv(DECOMP_LU): OpenCV's closed-form 3x3 inverse (cofactors times 1/det3) of K with R = I
     m = np.array([[fx, 0.0, cx], [0.0, fy, cy], [0.0, 0.0, 1.0]])
@@ -45,16 +66,7 @@ def undistort_map(width, height, fx, fy, cx, cy, d0=0.0, d1=0.0, d2=0.0, d3=0.0,
     kr = 1 + ((k3 * r2 + k2) * r2 + k1) * r2
     u = fx * (x * kr + p1 * _2xy + p2 * (r2 + 2 * x2)) + cx
     v = fy * (y * kr + p1 * (r2 + 2 * y2) + p2 * _2xy) + cy
-
-    def cv_round(t):  # cvRound: round half to even; out of int range (or NaN) gives INT_MIN like cvtsd2si
-        r = np.rint(t)
-        ok = (r >= -2147483648.0) & (r <= 2147483647.0)
-        return np.where(ok, np.where(ok, r, 0).astype(np.int64), -2147483648).astype(np.int64)
-
-    iu, iv = cv_round(u * 32), cv_round(v * 32)
-    map1 = np.stack([(iu >> 5).astype(np.int16), (iv >> 5).astype(np.int16)], -1)  # (short) cast: wraps like C
-    map2 = ((iv & 31) * 32 + (iu & 31)).astype(np.uint16)
-    return map1, map2
+    return u * 32, v * 32
 
 
 def remap_linear(img, map1, map2):
