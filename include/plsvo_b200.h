@@ -451,8 +451,9 @@ int plsvo_track_atan_batch_run(plsvo_ctx* ctx, const plsvo_atan_camera* cam, con
  *   plan lies within that of the limit is planned for the next kernel variant, as any batch that does not fit; with no
  *   variant left, or PLSVO_VARIANT pinned, it returns PLSVO_ERR_INVALID (DESIGN.md §4.11).
  * - Raw frames: plsvo_*_raw_multicam_batch_run above.
- * - ATAN (FOV) cameras per pair: plsvo_*_atan_multicam_batch_run below.
- * - Out of scope: a ragged (unpadded) frame layout, pinhole and ATAN pairs in one batch, the arrival-gated streamed path, separate upload / launch / download legs, dist.align_sharded, the seed updates
+ * - ATAN (FOV) cameras per pair: plsvo_*_atan_multicam_batch_run below.  Pinhole and ATAN pairs in one batch:
+ *   plsvo_*_any_camera_batch_run below.
+ * - Out of scope: a ragged (unpadded) frame layout, the arrival-gated streamed path, separate upload / launch / download legs, dist.align_sharded, the seed updates
  *   and the drop-in shim (one frame per call, nothing to batch).  Direct matching with a camera per image:
  *   plsvo_match_direct_multicam_batch_run.
  * ---------------------------------------------------------------------------------------- */
@@ -488,8 +489,9 @@ int plsvo_track_multicam_batch_run(plsvo_ctx* ctx, const plsvo_camera* cams /* [
  *   kernels returns PLSVO_ERR_CUDA.
  * - The kernels keep the pair's members, size and distortion terms in 128 bytes of shared memory per CTA, planned for as
  *   for the multicam kernels (DESIGN.md §4.14).
- * - Out of scope: pinhole and ATAN pairs in one batch, raw frames, the arrival-gated path, a ragged layout, the seed
- *   updates and the drop-in shim.  Direct matching with a camera per image: plsvo_match_direct_multicam_batch_run.
+ * - Pinhole and ATAN pairs in one batch: plsvo_*_any_camera_batch_run below.
+ * - Out of scope: raw frames, the arrival-gated path, a ragged layout, the seed updates and the drop-in shim.  Direct
+ *   matching with a camera per image: plsvo_match_direct_multicam_batch_run.
  * ---------------------------------------------------------------------------------------- */
 int plsvo_align_atan_multicam_batch_run(plsvo_ctx* ctx, const plsvo_atan_camera* cams /* [B] */, const plsvo_align_batch* batch,
                                         const plsvo_align_params* params, const plsvo_align_result* out);
@@ -653,6 +655,47 @@ int plsvo_match_direct_multicam_batch_run(plsvo_ctx* ctx, const plsvo_match_came
                                           const int32_t* cam_of_ref /* [n_ref_images] */,
                                           const int32_t* cam_of_cur /* [n_cur_images] */, const plsvo_match_batch* in,
                                           const plsvo_match_result* out);
+
+/* ------------------------------------------------------------------------------------------
+ * Any-camera batches: frame pairs from pinhole and ATAN (FOV) cameras in one call, e.g. rectified EuRoC / TUM streams next
+ * to SVO's 752x480 FOV camera.  These are plsvo_align_multicam_batch_run / plsvo_align_atan_multicam_batch_run (and the
+ * track calls) with pair b's camera, and its model, taken from a table: cams[cam_of_pair[b]], the records of
+ * plsvo_match_direct_multicam_batch_run, so that one camera table serves matching and alignment.
+ * - Slot: of batch->cam only width and height are used; they are the slot.  Pair b's frames are its camera's width x
+ *   height in the top-left corner of their slots, as for plsvo_align_multicam_batch_run.
+ * - The model tag decides the model, never the parameters: an ATAN camera with d0 = 0 stays ATAN (the two models do not
+ *   compute the same bits, DESIGN.md §4.10).  A pinhole camera is plsvo_camera in pixels; an ATAN camera is the
+ *   constructor's arguments, its members derived exactly as plsvo_align_atan_batch_run derives them.
+ * - Exactness: a pinhole pair's outputs are byte for byte those of plsvo_align_multicam_batch_run on that pair with that
+ *   camera's plsvo_camera; an ATAN pair's those of plsvo_align_atan_multicam_batch_run on that pair with that
+ *   plsvo_atan_camera; both at the same kernel variant.
+ * - Everything else of `batch` is as for those calls: full or lean bearings (lean ones formed with the pair's own model's
+ *   cam2world), depths, ragged counts and masks, NULL levels derived on the device, every kernel variant (PLSVO_VARIANT)
+ *   and PLSVO_ALIGN_FRAME_CHAIN, in which consecutive pairs need cameras of one size.
+ * - Track: frame b's errorMultiplier2 is |fx| of a pinhole camera and fx_ = width * fx of an ATAN camera; po_batch->fx is
+ *   ignored.
+ * - These calls always run upload -> launch -> download on the context's stream (not the arrival-gated path) and have
+ *   finished with the caller's arrays when they return, whatever they return.
+ * - NULL cams or cam_of_pair; n_cams < 1; a cam_of_pair[b] outside [0, n_cams); an unknown model; a camera of the table
+ *   that plsvo_align_multicam_batch_run (pinhole) or plsvo_align_atan_multicam_batch_run (ATAN) would reject — wider or
+ *   taller than the slot, below one pixel at a shipped or aligned level, non-finite or zero intrinsics; every camera of
+ *   the table is checked, and the camera index is in the message; a size change between consecutive pairs of a frame
+ *   chain (the pair indices are in the message); a batch <= 0; or (track) batch sizes that differ return
+ *   PLSVO_ERR_INVALID before anything is queued, and the context stays usable.  A library built without the any-camera
+ *   kernels returns PLSVO_ERR_CUDA.
+ * - The kernels keep the pair's camera, size, distortion terms and model tag in 128 bytes of shared memory per CTA,
+ *   planned for as for the multicam kernels (DESIGN.md §4.17).
+ * - Out of scope: raw (distorted pinhole) frames, the arrival-gated path, separate upload / launch / download legs,
+ *   dist.align_sharded, a ragged layout, the seed updates and the drop-in shim.
+ * ---------------------------------------------------------------------------------------- */
+int plsvo_align_any_camera_batch_run(plsvo_ctx* ctx, const plsvo_match_camera* cams, int32_t n_cams,
+                                     const int32_t* cam_of_pair /* [B] */, const plsvo_align_batch* batch,
+                                     const plsvo_align_params* params, const plsvo_align_result* out);
+int plsvo_track_any_camera_batch_run(plsvo_ctx* ctx, const plsvo_match_camera* cams, int32_t n_cams,
+                                     const int32_t* cam_of_pair /* [B] */, const plsvo_align_batch* al_batch,
+                                     const plsvo_align_params* al_params, const plsvo_poseopt_batch* po_batch,
+                                     const plsvo_poseopt_params* po_params, const plsvo_align_result* al_out,
+                                     const plsvo_poseopt_result* po_out);
 
 /* ---- Structure optimisation: Point::optimize / LineSeg::optimize (SURVEY.md §8f rank 3, "next") ---
  * Replaces, for a batch of 3D features, include/plsvo/feature3D.h:120,157 / src/feature3D_impl.cpp:36-95,

@@ -573,6 +573,11 @@ ABI_SYMBOLS = [
     ("plsvo_match_direct_atan_batch_run", C.c_int, [C.c_void_p, _P(AtanCamera), _P(MatchBatch), _P(MatchResult)]),
     ("plsvo_match_direct_multicam_batch_run", C.c_int, [C.c_void_p, _P(MatchCamera), C.c_int32, _P(C.c_int32), _P(C.c_int32),
                                                         _P(MatchBatch), _P(MatchResult)]),
+    ("plsvo_align_any_camera_batch_run", C.c_int, [C.c_void_p, _P(MatchCamera), C.c_int32, _P(C.c_int32), _P(AlignBatch),
+                                                   _P(AlignParams), _P(AlignResult)]),
+    ("plsvo_track_any_camera_batch_run", C.c_int, [C.c_void_p, _P(MatchCamera), C.c_int32, _P(C.c_int32), _P(AlignBatch),
+                                                   _P(AlignParams), _P(PoseOptBatch), _P(PoseOptParams), _P(AlignResult),
+                                                   _P(PoseOptResult)]),
     ("plsvo_seed_update_batch_run", C.c_int, [C.c_void_p, _P(SeedBatch), _P(SeedResult)]),
     ("plsvo_line_seed_update_batch_run", C.c_int, [C.c_void_p, _P(LineSeedBatch), _P(LineSeedResult)]),
     ("plsvo_structopt_batch_run", C.c_int, [C.c_void_p, _P(StructOptBatch), _P(StructOptResult)]),

@@ -124,10 +124,21 @@ class SparseImgAlign:
         each pair's frames sit in, top-left (synth.merge_sizes builds such a batch); data.cam's size for every pair
         when None.  cam_of_pair: [B] indices into `camera`, then a sequence of ATANCamera, when the pairs come from
         differently calibrated ATAN cameras (plsvo_align_atan_multicam_batch_run): pair b is aligned with
-        camera[cam_of_pair[b]], its frames that camera's size in the top-left corner of data.cam's slot."""
-        atan_cams = _atan_cameras_arg(camera, cameras, sizes, cam_of_pair, data)
+        camera[cam_of_pair[b]], its frames that camera's size in the top-left corner of data.cam's slot.  A sequence
+        that also holds undistorted pinhole cameras (synth.Camera) aligns pinhole and ATAN pairs in one call
+        (plsvo_align_any_camera_batch_run), each pair with its own camera's model."""
+        any_cams = _any_cameras_arg(camera, cameras, sizes, cam_of_pair, data)
+        atan_cams = None if any_cams else _atan_cameras_arg(camera, cameras, sizes, cam_of_pair, data)
         batch, keep = abi.make_align_batch(data)
         out = abi.AlignOut(data.batch, data.n_segs)
+        if any_cams:
+            cams, n_cams, cop = any_cams
+            self.ctx.check(self.ctx.lib.plsvo_align_any_camera_batch_run(self.ctx.handle, cams, n_cams,
+                                                                         cop.ctypes.data_as(C.POINTER(C.c_int32)), C.byref(batch),
+                                                                         C.byref(self.params), C.byref(out.struct)),
+                           "plsvo_align_any_camera_batch_run")
+            self.last = out
+            return out
         if atan_cams is not None:
             self.ctx.check(self.ctx.lib.plsvo_align_atan_multicam_batch_run(self.ctx.handle, atan_cams, C.byref(batch),
                                                                             C.byref(self.params), C.byref(out.struct)),
@@ -221,9 +232,11 @@ def track(align_data, poseopt_data, max_level: int = 4, min_level: int = 2, n_it
     sizes: with cameras, [B, 2] of every pair's (width, height), as for SparseImgAlign.run.
     cam_of_pair: with a sequence of ATANCamera as `camera`, as for SparseImgAlign.run
     (plsvo_track_atan_multicam_batch_run); frame b's errorMultiplier2 is then its camera's fx_ and poseopt_data.fx is
-    not used.
+    not used.  With pinhole cameras (synth.Camera) in the sequence too (plsvo_track_any_camera_batch_run), frame b's
+    errorMultiplier2 is |fx| of a pinhole camera and fx_ of an ATAN camera.
     Returns (AlignOut, PoseOptOut)."""
-    atan_cams = _atan_cameras_arg(camera, cameras, sizes, cam_of_pair, align_data)
+    any_cams = _any_cameras_arg(camera, cameras, sizes, cam_of_pair, align_data)
+    atan_cams = None if any_cams else _atan_cameras_arg(camera, cameras, sizes, cam_of_pair, align_data)
     ctx = ctx or default_context()
     ap = abi.align_params(max_level, min_level, n_iter)
     pp = abi.poseopt_params(reproj_thresh, po_n_iter, -1 if po_n_iter_ref is None else po_n_iter_ref)
@@ -233,6 +246,13 @@ def track(align_data, poseopt_data, max_level: int = 4, min_level: int = 2, n_it
         pb.T_f_w = abi._f64p()
     ao = abi.AlignOut(align_data.batch, align_data.n_segs)
     po = abi.PoseOptOut(poseopt_data.batch, poseopt_data.n_pts, poseopt_data.n_segs)
+    if any_cams:
+        cams, n_cams, cop = any_cams
+        ctx.check(ctx.lib.plsvo_track_any_camera_batch_run(ctx.handle, cams, n_cams, cop.ctypes.data_as(C.POINTER(C.c_int32)),
+                                                           C.byref(ab), C.byref(ap), C.byref(pb), C.byref(pp),
+                                                           C.byref(ao.struct), C.byref(po.struct)),
+                  "plsvo_track_any_camera_batch_run")
+        return ao, po
     if atan_cams is not None:
         ctx.check(ctx.lib.plsvo_track_atan_multicam_batch_run(ctx.handle, atan_cams, C.byref(ab), C.byref(ap), C.byref(pb),
                                                               C.byref(pp), C.byref(ao.struct), C.byref(po.struct)),
@@ -278,6 +298,30 @@ def _atan_cameras_arg(camera, cameras, sizes, cam_of_pair, data):
         return abi.make_atan_cameras([c.struct for c in camera], cam_of_pair, data.batch)
     except ValueError as e:
         raise PlsvoError(str(e)) from None
+
+
+def _any_cameras_arg(camera, cameras, sizes, cam_of_pair, data):
+    """(plsvo_match_camera[K], K, cam_of_pair as int32 [B]) of the any-camera calls when `camera` is a sequence of
+    ATANCamera and undistorted pinhole cameras (synth.Camera) with at least one of the latter, indexed by cam_of_pair;
+    None otherwise, for _atan_cameras_arg to handle (a sequence of ATANCamera only, or one holding anything else).  The
+    values (index ranges, camera sizes and parameters) are the C ABI's to check."""
+    import numpy as np
+
+    from .synth import Camera as UndistortedPinhole
+
+    if cam_of_pair is None or not isinstance(camera, (list, tuple)):
+        return None
+    if not any(isinstance(c, UndistortedPinhole) for c in camera):
+        return None
+    if not all(isinstance(c, (UndistortedPinhole, ATANCamera)) for c in camera):
+        return None
+    if cameras is not None or sizes is not None:
+        raise PlsvoError("cam_of_pair= selects a camera per pair: pass no cameras= or sizes= with it")
+    k = np.ascontiguousarray(cam_of_pair)
+    if k.shape != (data.batch,) or not np.issubdtype(k.dtype, np.integer):
+        raise PlsvoError(f"cam_of_pair must be integers of shape [{data.batch}], got {k.dtype} {list(k.shape)}")
+    k = k.astype(np.int32)
+    return abi.make_match_cameras(camera), len(camera), k
 
 
 def _cameras_arg(cameras, data, sizes=None):

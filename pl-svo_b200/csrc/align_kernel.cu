@@ -213,35 +213,44 @@ __device__ __forceinline__ bool cam_in_frame(int ox, int oy, int boundary, int l
 // positive by validation, and AlignArgs::fx holds fx_ for the ATAN kernels).
 // PinholePerPair is the undistorted pinhole with its own fx, fy, cx, cy for every pair (a.cams[b], the multicam entry
 // points): the same expressions as PinholeCam, with the intrinsics read from pair_intrinsics() instead of AlignArgs.
+// AnyPerPair is PinholePerPair or AtanPerPair, chosen per pair by the model tag a.cam_models[b] at run time.
 struct PinholeCam {  // vk::PinholeCamera without distortion
-  static constexpr bool kAtan = false, kPerPair = false;
+  static constexpr bool kAtan = false, kPerPair = false, kAny = false;
 };
 struct AtanCam {  // vk::ATANCamera, the FOV model (oracle/refdeps/vikit/atan_camera.h restates it)
-  static constexpr bool kAtan = true, kPerPair = false;
+  static constexpr bool kAtan = true, kPerPair = false, kAny = false;
 };
 struct PinholePerPair {  // vk::PinholeCamera without distortion, one per pair
-  static constexpr bool kAtan = false, kPerPair = true;
+  static constexpr bool kAtan = false, kPerPair = true, kAny = false;
 };
 struct AtanPerPair {  // vk::ATANCamera, one per pair: fx_..cy_ from a.cams[b], s_, s_inv_, tans_, tans_inv_ from a.atan_terms
-  static constexpr bool kAtan = true, kPerPair = true;
+  static constexpr bool kAtan = true, kPerPair = true, kAny = false;
+};
+// either of the two per-pair cameras: a.cams[b] as for both, a.atan_terms[b] read for ATAN pairs, a.cam_models[b] the tag.
+// kAtan is the compile-time model of the expressions, so it is false here; the tag picks them at run time.
+struct AnyPerPair {
+  static constexpr bool kAtan = false, kPerPair = true, kAny = true;
 };
 
 // fx, fy, cx, cy of the CTA's current pair (the per-pair cameras only), then its frame's width and height as two int32
-// in K[4], then (AtanPerPair) its distortion terms s_, s_inv_, tans_, tans_inv_ in K[5..8]: static shared memory, which
-// only the per-pair kernels instantiate.  The 40 (ATAN: 72) bytes cost 128 per CTA (the dynamic region behind them is
-// 128-byte aligned); the host plan reads the compiled size through align_multicam_kernel_static_smem /
-// align_atan_multicam_kernel_static_smem.  Thread 0 fills it from a.cams (and a.atan_terms) when the pair starts; every
-// use reads it back, as the pass reads ctl->dscale, so the camera and the size take no registers across the pass.
+// in K[4], then (AtanPerPair, AnyPerPair) its distortion terms s_, s_inv_, tans_, tans_inv_ in K[5..8], then
+// (AnyPerPair) its model tag as an int32 in K[9]: static shared memory, which only the per-pair kernels instantiate.  The
+// 40 (ATAN: 72, any: 80) bytes cost 128 per CTA (the dynamic region behind them is 128-byte aligned); the host plan reads
+// the compiled size through align_multicam_kernel_static_smem / align_atan_multicam_kernel_static_smem /
+// align_any_camera_kernel_static_smem.  Thread 0 fills it from a.cams (and a.atan_terms, a.cam_models) when the pair
+// starts; every use reads it back, as the pass reads ctl->dscale, so the camera and the size take no registers across
+// the pass.
 template <class Cam>
 __device__ __forceinline__ double* pair_intrinsics() {
   static_assert(Cam::kPerPair, "only the per-pair camera keeps its intrinsics in shared memory");
-  __shared__ double K[Cam::kAtan ? 9 : 5];
+  __shared__ double K[Cam::kAny ? 10 : Cam::kAtan ? 9 : 5];
   return K;
 }
-// s_, s_inv_, tans_, tans_inv_ of the CTA's current pair (AtanPerPair only)
+// s_, s_inv_, tans_, tans_inv_ of the CTA's current pair (AtanPerPair, and the ATAN pairs of AnyPerPair)
 template <class Cam>
 __device__ __forceinline__ const double* pair_atan_terms() {
-  static_assert(Cam::kAtan && Cam::kPerPair, "only the per-pair ATAN camera keeps its distortion terms in shared memory");
+  static_assert((Cam::kAtan || Cam::kAny) && Cam::kPerPair,
+                "only the per-pair ATAN camera keeps its distortion terms in shared memory");
   return pair_intrinsics<Cam>() + 5;
 }
 // The pair's frame size (width, height): the top-left corner of the batch's a.width x a.height slot it sits in.
@@ -249,14 +258,21 @@ template <class Cam>
 __device__ __forceinline__ int* pair_size() {
   return reinterpret_cast<int*>(pair_intrinsics<Cam>() + 4);
 }
+// The model tag of the CTA's current pair (AnyPerPair only): PLSVO_CAMERA_PINHOLE or PLSVO_CAMERA_ATAN
+template <class Cam>
+__device__ __forceinline__ int* pair_model() {
+  static_assert(Cam::kAny, "only the any-camera kernel keeps a model tag in shared memory");
+  return reinterpret_cast<int*>(pair_intrinsics<Cam>() + 9);
+}
 
 // cam2world: the constructors of PointFeat / LineFeat derive their bearing vectors this way (src/feature.cpp:42,98-99),
 // every operation rounded on its own (Eigen: x / sqrt(x.x)).
 //   pinhole: ((u-cx)/fx, (v-cy)/fy, 1).normalized()   (rpg_vikit pinhole_camera.cpp)
 //   ATAN:    d = ((u-cx_)/fx_, (v-cy_)/fy_), r_d = |d|, r = s_ ? tan(r_d s_) tans_inv_ : r_d,
 //            (factor d, 1).normalized() with factor = r_d > 0.01 ? r / r_d : 1
-template <class Cam>
-__device__ __forceinline__ void cam2world(const AlignArgs& a, const double* px, double* f) {
+// Atan: the model of the expressions (Cam::kAtan, or the pair's tag for AnyPerPair); Cam: where the camera is read.
+template <class Cam, bool Atan>
+__device__ __forceinline__ void cam2world_as(const AlignArgs& a, const double* px, double* f) {
   double x, y;
   if constexpr (Cam::kPerPair) {
     const double* K = pair_intrinsics<Cam>();
@@ -264,7 +280,7 @@ __device__ __forceinline__ void cam2world(const AlignArgs& a, const double* px, 
   } else {
     x = __ddiv_rn(__dsub_rn(px[0], a.cx), a.fx), y = __ddiv_rn(__dsub_rn(px[1], a.cy), a.fy);
   }
-  if constexpr (Cam::kAtan) {
+  if constexpr (Atan) {
     double s = a.atan_s, tans_inv = a.atan_tans_inv;
     if constexpr (Cam::kPerPair) s = pair_atan_terms<Cam>()[0], tans_inv = pair_atan_terms<Cam>()[3];
     const double rd = __dsqrt_rn(__dadd_rn(__dmul_rn(x, x), __dmul_rn(y, y)));
@@ -274,6 +290,16 @@ __device__ __forceinline__ void cam2world(const AlignArgs& a, const double* px, 
   }
   const double n = __dsqrt_rn(__dadd_rn(__dadd_rn(__dmul_rn(x, x), __dmul_rn(y, y)), 1.0));
   f[0] = __ddiv_rn(x, n), f[1] = __ddiv_rn(y, n), f[2] = __ddiv_rn(1.0, n);
+}
+// One pair runs per CTA at a time, so AnyPerPair's branch on the tag is uniform across the CTA.
+template <class Cam>
+__device__ __forceinline__ void cam2world(const AlignArgs& a, const double* px, double* f) {
+  if constexpr (Cam::kAny) {
+    if (*pair_model<Cam>() == PLSVO_CAMERA_ATAN) cam2world_as<Cam, true>(a, px, f);
+    else cam2world_as<Cam, false>(a, px, f);
+  } else {
+    cam2world_as<Cam, Cam::kAtan>(a, px, f);
+  }
 }
 
 // Rank-2 update of the 21 (upper-triangular H) + 6 (Jres) accumulators of one thread for a patch whose 3-D
@@ -320,16 +346,16 @@ __device__ __forceinline__ float row_px(uint32_t lo, uint32_t hi, int k) {
 // across the pass it would take 24 of the 128 registers of <128,4> and push the accumulators into local memory.
 // ATAN: world2cam(uv) with r = |uv|, factor = (r < 0.001 || s_ == 0) ? 1 : s_inv_ atan(r tans_) / r and
 // px = (cx_ + fx_ (factor u), cy_ + fy_ (factor v)), each of its operations rounded on its own.
-template <class Cam>
-__device__ __forceinline__ void project(const PairCtl* ctl, const AlignArgs& a, double xn, double yn, double zi, double& u,
-                                        double& v) {
+template <class Cam, bool Atan>
+__device__ __forceinline__ void project_as(const PairCtl* ctl, const AlignArgs& a, double xn, double yn, double zi, double& u,
+                                           double& v) {
   const double* R = ctl->R;
   const double* t = ctl->t;
   const double xc = R[0] * xn + R[1] * yn + (R[2] + t[0] * zi);
   const double yc = R[3] * xn + R[4] * yn + (R[5] + t[1] * zi);
   const double zc = R[6] * xn + R[7] * yn + (R[8] + t[2] * zi);
   const double izc = __drcp_rn(zc);
-  if constexpr (Cam::kAtan && Cam::kPerPair) {
+  if constexpr (Atan && Cam::kPerPair) {
     const double* K = pair_intrinsics<Cam>();
     const double* T = pair_atan_terms<Cam>();
     const double un = xc * izc, vn = yc * izc;
@@ -338,7 +364,7 @@ __device__ __forceinline__ void project(const PairCtl* ctl, const AlignArgs& a, 
     if (!(r < 0.001) && T[0] != 0.0) factor = __ddiv_rn(__dmul_rn(T[1], atan(__dmul_rn(r, T[2]))), r);
     u = __dadd_rn(K[2], __dmul_rn(K[0], __dmul_rn(factor, un))) * ctl->dscale;
     v = __dadd_rn(K[3], __dmul_rn(K[1], __dmul_rn(factor, vn))) * ctl->dscale;
-  } else if constexpr (Cam::kAtan) {
+  } else if constexpr (Atan) {
     const double un = xc * izc, vn = yc * izc;
     const double r = __dsqrt_rn(__dadd_rn(__dmul_rn(un, un), __dmul_rn(vn, vn)));
     double factor = 1.0;
@@ -352,6 +378,16 @@ __device__ __forceinline__ void project(const PairCtl* ctl, const AlignArgs& a, 
   } else {
     u = (a.fx * (xc * izc) + a.cx) * ctl->dscale;
     v = (a.fy * (yc * izc) + a.cy) * ctl->dscale;
+  }
+}
+template <class Cam>
+__device__ __forceinline__ void project(const PairCtl* ctl, const AlignArgs& a, double xn, double yn, double zi, double& u,
+                                        double& v) {
+  if constexpr (Cam::kAny) {
+    if (*pair_model<Cam>() == PLSVO_CAMERA_ATAN) project_as<Cam, true>(ctl, a, xn, yn, zi, u, v);
+    else project_as<Cam, false>(ctl, a, xn, yn, zi, u, v);
+  } else {
+    project_as<Cam, Cam::kAtan>(ctl, a, xn, yn, zi, u, v);
   }
 }
 // seven consecutive bytes (reference image, global memory, read-only path)
@@ -782,8 +818,9 @@ __device__ __forceinline__ void align_pairs(const AlignArgs& a) {
         const plsvo_camera& cam = a.cams[b];
         K[0] = cam.fx, K[1] = cam.fy, K[2] = cam.cx, K[3] = cam.cy;
         pair_size<Cam>()[0] = cam.width, pair_size<Cam>()[1] = cam.height;
-        if constexpr (Cam::kAtan)
+        if constexpr (Cam::kAtan || Cam::kAny)
           for (int i = 0; i < 4; ++i) K[5 + i] = a.atan_terms[4 * (size_t)b + i];
+        if constexpr (Cam::kAny) *pair_model<Cam>() = a.cam_models[b];
       }
     }
     // Host-buffer pipeline with lean inputs: pyramid levels above a.derive_from were not shipped; this CTA forms them
@@ -1438,6 +1475,11 @@ __global__ void __launch_bounds__(NT, MINB) sparse_img_align_atan_multicam_kerne
   align_pairs<NT, AtanPerPair>(a);
 }
 
+template <int NT, int MINB>
+__global__ void __launch_bounds__(NT, MINB) sparse_img_align_any_camera_kernel(const AlignArgs a) {
+  align_pairs<NT, AnyPerPair>(a);
+}
+
 }  // namespace
 
 namespace {
@@ -1633,6 +1675,54 @@ cudaError_t align_atan_multicam_kernel_launch(const AlignArgs& a, int grid, int 
 #define X(NT, MB)                                                                   \
   if (threads == NT && min_blocks == MB) {                                          \
     sparse_img_align_atan_multicam_kernel<NT, MB><<<grid, NT, smem_bytes, s>>>(a);  \
+    return cudaGetLastError();                                                      \
+  }
+  PLSVO_ALIGN_VARIANTS(X)
+#undef X
+  return cudaErrorInvalidValue;
+}
+
+// the same variants with a pinhole or ATAN camera per pair (a.cams, a.atan_terms, a.cam_models)
+namespace {
+template <int NT, int MINB>
+cudaError_t prepare_any_camera_t(size_t smem_bytes, int* ctas_per_sm) {
+  cudaError_t e = cudaFuncSetAttribute(sparse_img_align_any_camera_kernel<NT, MINB>,
+                                       cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_bytes);
+  if (e != cudaSuccess) return e;
+  e = cudaFuncSetAttribute(sparse_img_align_any_camera_kernel<NT, MINB>, cudaFuncAttributePreferredSharedMemoryCarveout,
+                           cudaSharedmemCarveoutMaxShared);
+  if (e != cudaSuccess) return e;
+  return cudaOccupancyMaxActiveBlocksPerMultiprocessor(ctas_per_sm, sparse_img_align_any_camera_kernel<NT, MINB>, NT,
+                                                       smem_bytes);
+}
+}  // namespace
+
+cudaError_t align_any_camera_kernel_prepare(int threads, int min_blocks, size_t smem_bytes, int* ctas_per_sm) {
+#define X(NT, MB) \
+  if (threads == NT && min_blocks == MB) return prepare_any_camera_t<NT, MB>(smem_bytes, ctas_per_sm);
+  PLSVO_ALIGN_VARIANTS(X)
+#undef X
+  return cudaErrorInvalidValue;
+}
+
+cudaError_t align_any_camera_kernel_static_smem(int threads, int min_blocks, size_t* bytes) {
+  cudaFuncAttributes fa;
+#define X(NT, MB)                                                                                \
+  if (threads == NT && min_blocks == MB) {                                                       \
+    const cudaError_t e = cudaFuncGetAttributes(&fa, sparse_img_align_any_camera_kernel<NT, MB>); \
+    *bytes = e == cudaSuccess ? fa.sharedSizeBytes : 0;                                          \
+    return e;                                                                                    \
+  }
+  PLSVO_ALIGN_VARIANTS(X)
+#undef X
+  return cudaErrorInvalidValue;
+}
+
+cudaError_t align_any_camera_kernel_launch(const AlignArgs& a, int grid, int threads, int min_blocks, size_t smem_bytes,
+                                              cudaStream_t s) {
+#define X(NT, MB)                                                                   \
+  if (threads == NT && min_blocks == MB) {                                          \
+    sparse_img_align_any_camera_kernel<NT, MB><<<grid, NT, smem_bytes, s>>>(a);  \
     return cudaGetLastError();                                                      \
   }
   PLSVO_ALIGN_VARIANTS(X)

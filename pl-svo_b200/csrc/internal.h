@@ -75,6 +75,9 @@ struct AlignArgs {
   // [B][4] s_, s_inv_, tans_, tans_inv_ of every pair's vk::ATANCamera (read by the ATAN multicam kernels only, instead
   // of atan_s..atan_tans_inv above; a.cams[b] then holds the pair's members fx_, fy_, cx_, cy_ and its size)
   const double* atan_terms;
+  // [B] model tag of every pair, PLSVO_CAMERA_PINHOLE or PLSVO_CAMERA_ATAN (read by the any-camera kernels only: a.cams[b]
+  // then holds a pinhole pair's fx..cy or an ATAN pair's members, and a.atan_terms[b] an ATAN pair's distortion terms)
+  const int32_t* cam_models;
 };
 
 // Opaque chi2 patches (16 float terms each) the alignment kernel can hold per Gauss-Newton pass: the patches whose 16
@@ -116,6 +119,14 @@ __attribute__((weak)) cudaError_t align_atan_multicam_kernel_prepare(int threads
                                                                      int* ctas_per_sm);
 __attribute__((weak)) cudaError_t align_atan_multicam_kernel_launch(const AlignArgs& a, int grid, int threads, int min_blocks,
                                                                     size_t smem_bytes, cudaStream_t s);
+// The same kernel variants with a pinhole or ATAN camera per pair, AlignArgs::cams, atan_terms and cam_models
+// (plsvo_align_any_camera_batch_run).  Weak for the same reason; their static shared memory (the pair's camera, size,
+// distortion terms and model tag, 80 bytes padded to 128 on sm_90a) is planned for as for the multicam kernels.
+__attribute__((weak)) cudaError_t align_any_camera_kernel_static_smem(int threads, int min_blocks, size_t* bytes);
+__attribute__((weak)) cudaError_t align_any_camera_kernel_prepare(int threads, int min_blocks, size_t smem_bytes,
+                                                                  int* ctas_per_sm);
+__attribute__((weak)) cudaError_t align_any_camera_kernel_launch(const AlignArgs& a, int grid, int threads, int min_blocks,
+                                                                 size_t smem_bytes, cudaStream_t s);
 
 // ---------------------------------------------------------------------------------------------
 struct PoseOptArgs {

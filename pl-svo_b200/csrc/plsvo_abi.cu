@@ -68,6 +68,8 @@ struct plsvo_ctx_impl {
   bool multicam = false;           // every pair has its own pinhole intrinsics, aa.cams (the multicam kernel variants)
   DevBuf d_cams;                   // plsvo_camera[B] of a multicam batch
   DevBuf d_atan_terms;             // [B][4] distortion terms of an ATAN multicam batch (aa.atan_terms)
+  bool any_camera = false;         // every pair has its own pinhole or ATAN camera, aa.cam_models (the any-camera variants)
+  DevBuf d_cam_models;             // [B] model tags of an any-camera batch (aa.cam_models)
   DevBuf d_feat;                     // every per-pair input array of the batch, at 256-byte-aligned offsets
   size_t feat_bytes = 0;
   char* h_po_out = nullptr;          // pinned staging of the pose-optimiser outputs (one D2H per download)
@@ -108,6 +110,7 @@ struct plsvo_ctx_impl {
   std::vector<std::unique_ptr<CamMap>> mc_maps;
   std::vector<plsvo_camera> h_mc_cams;  // plsvo_camera[B] of a raw or ATAN multicam call, staged for multicam_select
   std::vector<double> h_atan_terms;     // [B][4] distortion terms of an ATAN multicam call, staged for the upload
+  std::vector<int32_t> h_cam_models;    // [B] model tags of an any-camera call, staged for the upload
   std::vector<RawVisit> h_visit;        // the frames of a raw multicam call in camera-grouped order, with their maps
   DevBuf d_visit;
   DevBuf p_out_T;  // every pose-optimiser output, one block
@@ -376,8 +379,10 @@ int align_layout(plsvo_ctx_impl* c, const plsvo_align_batch* h) {
   c->chain = (h->flags & PLSVO_ALIGN_FRAME_CHAIN) != 0;
   c->atan = false;  // the ATAN entry points set it after the upload
   c->multicam = false;  // and so do the multicam entry points
+  c->any_camera = false;  // and the any-camera entry points
   a.cams = nullptr;
   a.atan_terms = nullptr;
+  a.cam_models = nullptr;
   a.B = h->batch, a.n_pts = h->n_pts, a.n_segs = h->n_segs;
   a.width = h->cam.width, a.height = h->cam.height;
   a.fx = h->cam.fx, a.fy = h->cam.fy, a.cx = h->cam.cx, a.cy = h->cam.cy;
@@ -825,12 +830,14 @@ int align_plan(plsvo_ctx_impl* c, const plsvo_align_params* p, AlignPlan* plan, 
       rc_last = fail(c, PLSVO_ERR_INVALID, "a segment has more than 1024 samples");
       continue;
     }
-    // static shared memory of the kernel, taken per CTA next to the dynamic plan below: the multicam kernels (pinhole
-    // and ATAN) hold their pair's camera there (with the alignment of the dynamic region behind them); the others have none
+    // static shared memory of the kernel, taken per CTA next to the dynamic plan below: the multicam kernels (pinhole,
+    // ATAN and any camera) hold their pair's camera there (with the alignment of the dynamic region behind them); the
+    // others have none
     size_t static_smem = 0;
     if (c->multicam)
-      CK(c->atan ? align_atan_multicam_kernel_static_smem(threads, min_blocks, &static_smem)
-                 : align_multicam_kernel_static_smem(threads, min_blocks, &static_smem));
+      CK(c->any_camera ? align_any_camera_kernel_static_smem(threads, min_blocks, &static_smem)
+         : c->atan     ? align_atan_multicam_kernel_static_smem(threads, min_blocks, &static_smem)
+                       : align_multicam_kernel_static_smem(threads, min_blocks, &static_smem));
     // shared-memory plan: stage the current image level when the CTA still fits min_blocks times per SM next to
     // the per-pair state; bigger levels are read through L2 with the same aligned-word loads.
     const int other = (int)(align_smem_bytes(a.n_pts, a.n_segs, a.max_patches, a.max_seg_slots, 0, threads) + static_smem);
@@ -863,7 +870,8 @@ int align_plan(plsvo_ctx_impl* c, const plsvo_align_params* p, AlignPlan* plan, 
     a.smem_img_bytes = img_bytes;
     a.rec_cap = rec_cap;
     int ctas_per_sm = 0;
-    CK(c->atan && c->multicam ? align_atan_multicam_kernel_prepare(threads, min_blocks, smem, &ctas_per_sm)
+    CK(c->any_camera          ? align_any_camera_kernel_prepare(threads, min_blocks, smem, &ctas_per_sm)
+       : c->atan && c->multicam ? align_atan_multicam_kernel_prepare(threads, min_blocks, smem, &ctas_per_sm)
        : c->atan              ? align_atan_kernel_prepare(threads, min_blocks, smem, &ctas_per_sm)
        : c->multicam          ? align_multicam_kernel_prepare(threads, min_blocks, smem, &ctas_per_sm)
                               : align_kernel_prepare(threads, min_blocks, smem, &ctas_per_sm));
@@ -903,7 +911,8 @@ int align_launch_kernel(plsvo_ctx_impl* c, const AlignPlan& plan, cudaStream_t s
   a.gate_chunk = gate_chunk;
   const int grid = std::min(a.B, c->num_sms * plan.ctas_per_sm);
   CK(cudaMemsetAsync(a.work_counter, 0, sizeof(unsigned int), s));
-  CK(c->atan && c->multicam ? align_atan_multicam_kernel_launch(a, grid, plan.threads, plan.min_blocks, plan.smem, s)
+  CK(c->any_camera          ? align_any_camera_kernel_launch(a, grid, plan.threads, plan.min_blocks, plan.smem, s)
+     : c->atan && c->multicam ? align_atan_multicam_kernel_launch(a, grid, plan.threads, plan.min_blocks, plan.smem, s)
      : c->atan              ? align_atan_kernel_launch(a, grid, plan.threads, plan.min_blocks, plan.smem, s)
      : c->multicam          ? align_multicam_kernel_launch(a, grid, plan.threads, plan.min_blocks, plan.smem, s)
                             : align_kernel_launch(a, grid, plan.threads, plan.min_blocks, plan.smem, s));
@@ -1650,6 +1659,127 @@ int plsvo_track_atan_multicam_batch_run(plsvo_ctx* ctx, const plsvo_atan_camera*
                                         const plsvo_poseopt_result* po) {
   if (!ctx || !ab || !ap || !pb || !pp || !po) return PLSVO_ERR_INVALID;
   return settled(CTX(ctx), track_atan_multicam_body(ctx, cams, ab, ap, pb, pp, ao, po));
+}
+
+}  // extern "C"
+
+// ------------------------------------------------------------------------------------------------
+// Any-camera batches: a pinhole or ATAN camera per pair, from a table of plsvo_match_camera
+// ------------------------------------------------------------------------------------------------
+namespace {
+
+// The camera table of an any-camera call, expanded per pair into the arrays the per-pair kernels read: c->h_mc_cams
+// (plsvo_camera records: a pinhole's fx..cy as given, an ATAN camera's members from atan_members), c->h_atan_terms
+// ([B][4], filled for ATAN pairs only) and c->h_cam_models ([B] tags).  Every camera of the table is checked against the
+// batch by multicam_check (slot, size, levels, intrinsics; the camera index in the message), then the per-pair records
+// for the rule that spans pairs (one size along a frame chain; the pair index in the message).  Nothing is queued here.
+int any_camera_check(plsvo_ctx_impl* c, const plsvo_match_camera* cams, int32_t n_cams, const int32_t* cam_of_pair,
+                     const plsvo_align_batch* b, const plsvo_align_params* p) {
+  if (!cams || !cam_of_pair) return fail(c, PLSVO_ERR_INVALID, "cams or cam_of_pair is NULL");
+  if (n_cams < 1) return fail(c, PLSVO_ERR_INVALID, "n_cams must be at least 1");
+  if (b->batch <= 0) return fail(c, PLSVO_ERR_INVALID, "batch/n_pts/n_segs out of range");
+  char msg[160];
+  std::vector<plsvo_camera> recs((size_t)n_cams);
+  std::vector<double> terms(4 * (size_t)n_cams, 0.0);
+  for (int k = 0; k < n_cams; ++k) {
+    const plsvo_match_camera& m = cams[k];
+    if (m.model == PLSVO_CAMERA_PINHOLE) {
+      recs[k] = m.pinhole;
+    } else if (m.model == PLSVO_CAMERA_ATAN) {
+      // the size first: the derived focal lengths of a camera below one pixel would be reported instead
+      if (camera_fits_slot(c, k, m.atan.width, m.atan.height, b) != PLSVO_OK) return PLSVO_ERR_INVALID;
+      if (const char* why = atan_members(m.atan, &recs[k], &terms[4 * (size_t)k])) {
+        snprintf(msg, sizeof msg, "cams[%d] (ATAN) %s", k, why);
+        return fail(c, PLSVO_ERR_INVALID, msg);
+      }
+    } else {
+      snprintf(msg, sizeof msg, "cams[%d].model %d is neither PLSVO_CAMERA_PINHOLE nor PLSVO_CAMERA_ATAN", k, m.model);
+      return fail(c, PLSVO_ERR_INVALID, msg);
+    }
+  }
+  plsvo_align_batch table = *b;
+  table.batch = n_cams;
+  table.flags &= ~PLSVO_ALIGN_FRAME_CHAIN;  // the table's cameras are not a chain; the pairs are, below
+  int rc = multicam_check(c, recs.data(), &table, p);
+  if (rc != PLSVO_OK) return rc;
+  const size_t B = (size_t)b->batch;
+  c->h_mc_cams.resize(B);
+  c->h_atan_terms.assign(4 * B, 0.0);
+  c->h_cam_models.resize(B);
+  for (size_t i = 0; i < B; ++i) {
+    const int k = cam_of_pair[i];
+    if (k < 0 || k >= n_cams) {
+      snprintf(msg, sizeof msg, "cam_of_pair[%d] = %d is outside [0, %d)", (int)i, k, n_cams);
+      return fail(c, PLSVO_ERR_INVALID, msg);
+    }
+    c->h_mc_cams[i] = recs[k];
+    c->h_cam_models[i] = cams[k].model;
+    if (cams[k].model == PLSVO_CAMERA_ATAN) std::copy(&terms[4 * (size_t)k], &terms[4 * (size_t)k + 4], &c->h_atan_terms[4 * i]);
+  }
+  rc = multicam_check(c, c->h_mc_cams.data(), b, p);
+  if (rc == PLSVO_OK && (!align_any_camera_kernel_prepare || !align_any_camera_kernel_launch || !align_any_camera_kernel_static_smem))
+    rc = fail(c, PLSVO_ERR_CUDA, "this library was built without the any-camera alignment kernels");
+  return rc;
+}
+
+// after the upload of the alignment batch: the pairs' records, distortion terms and model tags follow it on the same
+// stream, and the any-camera kernels run the batch
+int any_camera_select(plsvo_ctx_impl* c) {
+  int rc = atan_multicam_select(c);
+  if (rc != PLSVO_OK) return rc;
+  CK(up(c->d_cam_models, c->h_cam_models.data(), c->h_cam_models.size(), c->stream, &c->aa.cam_models));
+  c->any_camera = true;
+  return PLSVO_OK;
+}
+
+}  // namespace
+
+extern "C" {
+
+static int align_any_camera_body(plsvo_ctx* ctx, const plsvo_match_camera* cams, int32_t n_cams, const int32_t* cam_of_pair,
+                                 const plsvo_align_batch* b, const plsvo_align_params* p, const plsvo_align_result* o) {
+  plsvo_ctx_impl* c = CTX(ctx);
+  int rc = any_camera_check(c, cams, n_cams, cam_of_pair, b, p);
+  if (rc == PLSVO_OK) rc = plsvo_align_upload(ctx, b);
+  if (rc == PLSVO_OK) rc = any_camera_select(c);
+  if (rc == PLSVO_OK) rc = plsvo_align_launch(ctx, p);
+  if (rc == PLSVO_OK) rc = plsvo_align_download(ctx, o);
+  return rc;
+}
+
+int plsvo_align_any_camera_batch_run(plsvo_ctx* ctx, const plsvo_match_camera* cams, int32_t n_cams, const int32_t* cam_of_pair,
+                                     const plsvo_align_batch* b, const plsvo_align_params* p, const plsvo_align_result* o) {
+  if (!ctx || !b || !p || !o) return PLSVO_ERR_INVALID;
+  return settled(CTX(ctx), align_any_camera_body(ctx, cams, n_cams, cam_of_pair, b, p, o));
+}
+
+static int track_any_camera_body(plsvo_ctx* ctx, const plsvo_match_camera* cams, int32_t n_cams, const int32_t* cam_of_pair,
+                                 const plsvo_align_batch* ab, const plsvo_align_params* ap, const plsvo_poseopt_batch* pb,
+                                 const plsvo_poseopt_params* pp, const plsvo_align_result* ao, const plsvo_poseopt_result* po) {
+  plsvo_ctx_impl* c = CTX(ctx);
+  int rc = any_camera_check(c, cams, n_cams, cam_of_pair, ab, ap);
+  if (rc == PLSVO_OK && pb->batch != ab->batch)
+    rc = fail(c, PLSVO_ERR_INVALID, "alignment and pose-optimiser batches differ in size");
+  if (rc == PLSVO_OK) rc = multicam_kernels_present(c, false, true);
+  if (rc != PLSVO_OK) return rc;
+  // the pose optimiser of frame b reads its camera's errorMultiplier2(): |fx| of a pinhole, fx_ (positive) of an ATAN camera
+  c->h_po_fx.resize((size_t)ab->batch);
+  for (int i = 0; i < ab->batch; ++i) c->h_po_fx[i] = fabs(c->h_mc_cams[i].fx);
+  rc = plsvo_track_upload(ctx, ab, pb);
+  if (rc == PLSVO_OK) rc = any_camera_select(c);
+  if (rc == PLSVO_OK) rc = poseopt_fx_select(c, c->h_po_fx.data());
+  if (rc == PLSVO_OK) rc = plsvo_track_launch(ctx, ap, pp);
+  if (rc == PLSVO_OK && ao) rc = plsvo_align_download(ctx, ao);
+  if (rc == PLSVO_OK) rc = plsvo_poseopt_download(ctx, po);
+  return rc;
+}
+
+int plsvo_track_any_camera_batch_run(plsvo_ctx* ctx, const plsvo_match_camera* cams, int32_t n_cams, const int32_t* cam_of_pair,
+                                     const plsvo_align_batch* ab, const plsvo_align_params* ap, const plsvo_poseopt_batch* pb,
+                                     const plsvo_poseopt_params* pp, const plsvo_align_result* ao,
+                                     const plsvo_poseopt_result* po) {
+  if (!ctx || !ab || !ap || !pb || !pp || !po) return PLSVO_ERR_INVALID;
+  return settled(CTX(ctx), track_any_camera_body(ctx, cams, n_cams, cam_of_pair, ab, ap, pb, pp, ao, po));
 }
 
 }  // extern "C"

@@ -662,6 +662,40 @@ def make_atan_multicam_batch(cams, cam_of_pair, slot: Camera | None = None, fill
     return al, scatter_batches(po_parts, index, len(cam_of_pair)), al_parts, po_parts, index
 
 
+def make_any_camera_batch(cams, cam_of_pair, slot: Camera | None = None, fill=0, poseopt: bool = False, n_pts: int = 300,
+                          n_segs: int = 80, seed: int = 3000, **align_kw):
+    """A batch of pairs from pinhole and ATAN (FOV) cameras (a sequence of Camera, the undistorted pinhole, and
+    api.ATANCamera), of one size or several: pair b is rendered and its features are lifted through cams[cam_of_pair[b]]
+    with that camera's own model at its own size (make_align_batch, with atan= for an ATAN camera; make_track_batch when
+    `poseopt`).  The per-camera parts are padded into one slot batch with merge_sizes (slot, fill as there).  Returns
+    what make_atan_multicam_batch returns: (AlignData, parts, groups), or (AlignData, PoseOptData, parts, po_parts,
+    groups) when `poseopt`, parts[i] and groups[i] those of the i-th camera that has pairs.  The pose optimiser of frame b
+    then takes errorMultiplier2 = |fx| of a pinhole camera, fx_ of an ATAN camera."""
+    cam_of_pair = np.asarray(cam_of_pair)
+    groups = [np.flatnonzero(cam_of_pair == k) for k in range(len(cams))]
+    used = [k for k in range(len(cams)) if len(groups[k])]
+    al_parts, po_parts = [], []
+    for k in used:
+        a = cams[k]
+        if isinstance(a, Camera):
+            cam, model = a, {}
+        else:
+            cam, model = Camera(a.width, a.height, a.fx_, a.fy_, a.cx_, a.cy_), {"atan": a}
+        kw = dict(cam=cam, batch=len(groups[k]), n_pts=n_pts, n_segs=n_segs, seed=seed + 104729 * k, **model, **align_kw)
+        if poseopt:
+            al, po = make_track_batch(**kw)
+            po.fx = abs(a.fx) if isinstance(a, Camera) else a.errorMultiplier2()
+            po_parts.append(po)
+        else:
+            al = make_align_batch(**kw)
+        al_parts.append(al)
+    index = [groups[k] for k in used]
+    al, _ = merge_sizes(al_parts, index, slot=slot, fill=fill)
+    if not poseopt:
+        return al, al_parts, index
+    return al, scatter_batches(po_parts, index, len(cam_of_pair)), al_parts, po_parts, index
+
+
 def make_sequence(cam: Camera = VGA, n_seq: int = 4, n_frames: int = 20, n_pts: int = 300, n_segs: int = 80, seed: int = 1000,
                   device: str | torch.device = "cpu", noise_px: float = 0.3, outlier_frac: float = 0.05):
     """BASELINE config 1 / SURVEY 8d C1: n_seq independent sequences of n_frames views along the smooth trajectory
