@@ -366,7 +366,8 @@ int plsvo_track_raw_batch_run(plsvo_ctx* ctx, const plsvo_raw_frames* raw, const
  *   belongs to two pairs), and everything the raw calls reject return PLSVO_ERR_INVALID before anything is queued.  A library built without the
  *   multicam kernels returns PLSVO_ERR_CUDA.  The calls always run upload -> launch -> download and have finished with
  *   the caller's arrays when they return, whatever they return.
- * - Out of scope: a ragged (unpadded) frame layout, ATAN cameras, frame chains, the arrival-gated path.
+ * - Lenses and ATAN (FOV) cameras in one batch: plsvo_*_raw_any_camera_batch_run below.
+ * - Out of scope: a ragged (unpadded) frame layout, frame chains, the arrival-gated path.
  * ---------------------------------------------------------------------------------------- */
 typedef struct plsvo_raw_multicam_frames {
   int32_t n_cams, reserved;
@@ -685,8 +686,9 @@ int plsvo_match_direct_multicam_batch_run(plsvo_ctx* ctx, const plsvo_match_came
  *   kernels returns PLSVO_ERR_CUDA.
  * - The kernels keep the pair's camera, size, distortion terms and model tag in 128 bytes of shared memory per CTA,
  *   planned for as for the multicam kernels (DESIGN.md §4.17).
- * - Out of scope: raw (distorted pinhole) frames, the arrival-gated path, separate upload / launch / download legs,
- *   dist.align_sharded, a ragged layout, the seed updates and the drop-in shim.
+ * - Raw (distorted pinhole) frames next to ATAN frames: plsvo_*_raw_any_camera_batch_run below.
+ * - Out of scope: the arrival-gated path, separate upload / launch / download legs, dist.align_sharded, a ragged layout,
+ *   the seed updates and the drop-in shim.
  * ---------------------------------------------------------------------------------------- */
 int plsvo_align_any_camera_batch_run(plsvo_ctx* ctx, const plsvo_match_camera* cams, int32_t n_cams,
                                      const int32_t* cam_of_pair /* [B] */, const plsvo_align_batch* batch,
@@ -696,6 +698,68 @@ int plsvo_track_any_camera_batch_run(plsvo_ctx* ctx, const plsvo_match_camera* c
                                      const plsvo_align_params* al_params, const plsvo_poseopt_batch* po_batch,
                                      const plsvo_poseopt_params* po_params, const plsvo_align_result* al_out,
                                      const plsvo_poseopt_result* po_out);
+
+/* ------------------------------------------------------------------------------------------
+ * Raw any-camera batches: raw frames from distorted pinhole lenses and from ATAN (FOV) cameras in one call, e.g. raw
+ * EuRoC / TUM streams next to SVO's 752x480 FOV camera.  Pair b's camera is cams[cam_of_pair[b]], and its tag picks
+ * what happens to both of the pair's frames:
+ *   PLSVO_CAMERA_PINHOLE: `pinhole` is the distorted lens, as for plsvo_undistort_batch; fabs(d0) <= 1e-7 means no
+ *     distortion.
+ *     The frames are rectified on the device with that lens's map and aligned as an undistorted pinhole with its fx, fy,
+ *     cx, cy: what plsvo_align_raw_multicam_batch_run does for that pair.
+ *   PLSVO_CAMERA_ATAN: `atan` is the constructor's arguments, as plsvo_align_atan_batch_run.  The frames are used as they
+ *     are (the pipeline never rectifies FOV frames), half-sampled into their pyramid and aligned through the ATAN model:
+ *     what plsvo_align_atan_multicam_batch_run does with that pair's pyramid.
+ * One fused rectify / pyramid kernel runs over every frame, then one alignment kernel (and, track, the pose optimiser).
+ * - Slot: as for plsvo_align_raw_multicam_batch_run, of batch->cam only width and height are used.  Every camera fits in
+ *   the slot, and a pair's frames sit in the top-left corner of their slots (raw stacks at `pitch` and `stride`).
+ * - The tag decides the model, never the parameters: a lens with d0 = 0 is a pinhole that copies its frame; an ATAN
+ *   camera with d0 = 0 stays ATAN.
+ * - Exactness, at the same kernel variant: a lens pair's outputs are byte for byte those of
+ *   plsvo_align_raw_multicam_batch_run on that pair with that lens; an ATAN pair's those of
+ *   plsvo_align_atan_multicam_batch_run on that pair with that camera, its levels createImgPyramid of its raw frames.
+ *   Equivalently, feeding rect_out to plsvo_align_any_camera_batch_run, with the table mapped to plsvo_match_camera
+ *   records (a lens becomes the undistorted pinhole of its fx..cy), gives the same bytes for every pair.
+ * - Track: frame b's errorMultiplier2 is |fx| of a lens and fx_ = width * fx of an ATAN camera; po_batch->fx is ignored.
+ * - rect_out as for the raw calls: every non-NULL level, the B reference frames followed by the B current frames, each
+ *   holding the pyramid the pipeline builds (rectified for a lens, the frame itself for an ATAN camera) in its slot's
+ *   region, the rest of the slot 0.
+ * - Maps: only distorted lenses build maps.  These calls share the cache of the raw multicam calls and its rule: after a
+ *   call it holds exactly the maps of the distorted lenses that call referenced.  plsvo_last_map_build_ms works as there.
+ * - NULL cams or cam_of_pair; n_cams < 1; a cam_of_pair[b] outside [0, n_cams); an unknown model; a table camera that
+ *   plsvo_align_raw_multicam_batch_run (lens) or plsvo_align_any_camera_batch_run (ATAN) would reject, every camera of the
+ *   table checked, used or not; a level (aligned or asked of rect_out) below one pixel for a camera some pair
+ *   references; PLSVO_ALIGN_FRAME_CHAIN; image pointers in `batch`; max_level > 6; or (track) batch sizes that differ
+ *   return PLSVO_ERR_INVALID, with the camera or pair index in the message, before anything is queued, and the context
+ *   stays usable.  A library built without the fused multicam launcher or the any-camera kernels returns PLSVO_ERR_CUDA.
+ * - These calls always run upload -> launch -> download on the context's stream (not the arrival-gated path) and have
+ *   finished with the caller's arrays when they return, whatever they return.
+ * - Out of scope: frame chains (a chained frame belongs to two pairs), the arrival-gated path, separate upload / launch /
+ *   download legs, a ragged layout, the seed updates and the drop-in shim, rectifying ATAN frames.
+ * ---------------------------------------------------------------------------------------- */
+typedef struct plsvo_raw_camera {
+  int32_t model, reserved;        /* PLSVO_CAMERA_PINHOLE or PLSVO_CAMERA_ATAN */
+  plsvo_pinhole_camera pinhole;   /* PINHOLE: the distorted lens, as for plsvo_undistort_batch; fabs(d0) <= 1e-7: no distortion */
+  plsvo_atan_camera atan;         /* ATAN: the constructor's arguments, as plsvo_align_atan_batch_run */
+} plsvo_raw_camera;
+
+typedef struct plsvo_raw_any_camera_frames {
+  int32_t n_cams, reserved;
+  const plsvo_raw_camera* cams;   /* [n_cams] */
+  const int32_t* cam_of_pair;     /* [B] index into cams: the camera of both frames of pair b */
+  const uint8_t* ref_raw;         /* [B] raw frames, one slot (batch->cam's size) each */
+  const uint8_t* cur_raw;         /* [B] raw frames, one slot (batch->cam's size) each */
+  size_t pitch, stride;           /* host layout of both stacks, as plsvo_raw_multicam_frames */
+} plsvo_raw_any_camera_frames;
+
+int plsvo_align_raw_any_camera_batch_run(plsvo_ctx* ctx, const plsvo_raw_any_camera_frames* raw, const plsvo_align_batch* batch,
+                                         const plsvo_align_params* params, const plsvo_align_result* out,
+                                         const plsvo_pyramid_result* rect_out);
+int plsvo_track_raw_any_camera_batch_run(plsvo_ctx* ctx, const plsvo_raw_any_camera_frames* raw,
+                                         const plsvo_align_batch* al_batch, const plsvo_align_params* al_params,
+                                         const plsvo_poseopt_batch* po_batch, const plsvo_poseopt_params* po_params,
+                                         const plsvo_align_result* al_out, const plsvo_poseopt_result* po_out,
+                                         const plsvo_pyramid_result* rect_out);
 
 /* ---- Structure optimisation: Point::optimize / LineSeg::optimize (SURVEY.md §8f rank 3, "next") ---
  * Replaces, for a batch of 3D features, include/plsvo/feature3D.h:120,157 / src/feature3D_impl.cpp:36-95,

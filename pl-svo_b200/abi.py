@@ -201,6 +201,66 @@ def make_match_cameras(cameras):
     return arr
 
 
+class RawCamera(C.Structure):
+    """plsvo_raw_camera: one camera of plsvo_align_raw_any_camera_batch_run, a distorted pinhole lens (the
+    vk::PinholeCamera constructor arguments) or an ATAN camera (its constructor arguments), chosen by `model`."""
+    _fields_ = [("model", C.c_int32), ("reserved", C.c_int32), ("pinhole", PinholeCamera), ("atan", AtanCamera)]
+
+
+class RawAnyCameraFrames(C.Structure):
+    """plsvo_raw_any_camera_frames: the camera table, the camera of every pair and the raw frame stacks of
+    plsvo_align_raw_any_camera_batch_run / plsvo_track_raw_any_camera_batch_run."""
+    _fields_ = [("n_cams", C.c_int32), ("reserved", C.c_int32), ("cams", C.POINTER(RawCamera)),
+                ("cam_of_pair", C.POINTER(C.c_int32)), ("ref_raw", _u8p), ("cur_raw", _u8p), ("pitch", C.c_size_t),
+                ("stride", C.c_size_t)]
+
+
+def make_raw_cameras(cameras):
+    """plsvo_raw_camera[K] from a sequence of api.PinholeCamera (distorted lens) / api.ATANCamera objects."""
+    arr = (RawCamera * len(cameras))()
+    for k, cam in enumerate(cameras):
+        if isinstance(cam.struct, AtanCamera):
+            arr[k].model, arr[k].atan = CAMERA_ATAN, cam.struct
+        elif isinstance(cam.struct, PinholeCamera):
+            arr[k].model, arr[k].pinhole = CAMERA_PINHOLE, cam.struct
+        else:
+            raise ValueError(f"raw camera table: entry {k} is neither a PinholeCamera nor an ATANCamera")
+    return arr
+
+
+def raw_to_match_cameras(table):
+    """The plsvo_match_camera[K] records of a raw camera table (RawCamera[K]), for the matching and any-camera calls on
+    the frames it produced: a lens becomes the undistorted pinhole of its size and fx..cy, an ATAN camera stays as it is."""
+    arr = (MatchCamera * len(table))()
+    for k, r in enumerate(table):
+        arr[k].model = r.model
+        if r.model == CAMERA_PINHOLE:
+            p = r.pinhole
+            arr[k].pinhole = Camera(p.width, p.height, 0, 0, p.fx, p.fy, p.cx, p.cy)
+        else:
+            arr[k].atan = r.atan
+    return arr
+
+
+def make_raw_any_camera_frames(table, cam_of_pair, raw, batch: int, slot):
+    """plsvo_raw_any_camera_frames for `batch` pairs: table, a RawCamera[K] (make_raw_cameras) whose cameras each fit the
+    slot; cam_of_pair, the index of every pair's camera; raw, a (ref, cur) pair of u8 [B,H,W] stacks of the slot's size
+    with the same strides (rows may be padded), frame b in the top-left corner of its slot.  slot: anything with a width
+    and a height (the batch's camera).  Returns (struct, keepalive)."""
+    if not isinstance(raw, (tuple, list)):
+        raise ValueError("raw any-camera frames: a (ref, cur) pair of [B,H,W] stacks (frame chains are not supported)")
+    if len(table) < 1:
+        raise ValueError("raw any-camera frames: at least one camera")
+    k = np.ascontiguousarray(cam_of_pair, dtype=np.int32)
+    if k.shape != (batch,):
+        raise ValueError(f"cam_of_pair must have shape [{batch}], got {list(k.shape)}")
+    frame = PinholeCamera()
+    frame.width, frame.height = slot.width, slot.height
+    r, _, stacks = make_raw_frames(frame, raw, batch)
+    m = RawAnyCameraFrames(len(table), 0, table, k.ctypes.data_as(C.POINTER(C.c_int32)), r.ref_raw, r.cur_raw, r.pitch, r.stride)
+    return m, (table, k, stacks)
+
+
 def make_cameras(cameras, cam, batch: int, sizes=None):
     """plsvo_camera[B] of a multicam call from `cameras`, an array-like [B, 4] of (fx, fy, cx, cy) rows.  Each has the
     image size of `cam` (the batch's camera, whose size is the slot every pair's frames sit in), or with `sizes`, an
@@ -556,6 +616,11 @@ ABI_SYMBOLS = [
     ("plsvo_track_raw_multicam_batch_run", C.c_int, [C.c_void_p, _P(RawMulticamFrames), _P(AlignBatch), _P(AlignParams),
                                                      _P(PoseOptBatch), _P(PoseOptParams), _P(AlignResult), _P(PoseOptResult),
                                                      _P(PyramidResult)]),
+    ("plsvo_align_raw_any_camera_batch_run", C.c_int, [C.c_void_p, _P(RawAnyCameraFrames), _P(AlignBatch), _P(AlignParams),
+                                                       _P(AlignResult), _P(PyramidResult)]),
+    ("plsvo_track_raw_any_camera_batch_run", C.c_int, [C.c_void_p, _P(RawAnyCameraFrames), _P(AlignBatch), _P(AlignParams),
+                                                       _P(PoseOptBatch), _P(PoseOptParams), _P(AlignResult), _P(PoseOptResult),
+                                                       _P(PyramidResult)]),
     ("plsvo_align_atan_batch_run", C.c_int, [C.c_void_p, _P(AtanCamera), _P(AlignBatch), _P(AlignParams), _P(AlignResult)]),
     ("plsvo_track_atan_batch_run", C.c_int, [C.c_void_p, _P(AtanCamera), _P(AlignBatch), _P(AlignParams), _P(PoseOptBatch),
                                              _P(PoseOptParams), _P(AlignResult), _P(PoseOptResult)]),

@@ -177,11 +177,16 @@ class SparseImgAlign:
         calibrated lenses (plsvo_align_raw_multicam_batch_run): pair b is rectified with camera[cam_of_pair[b]] and
         aligned with its fx, fy, cx, cy.  data.cam gives only the image size of the slot every frame sits in; a camera
         may be smaller, and its frames then occupy its own size in the top-left corner of their slots (of the raw
-        stacks and of the rect_levels arrays, whose rest is 0).  raw must then be a (ref, cur) pair of stacks."""
-        rf, batch, keep = _raw_call_args(camera, raw, data, cam_of_pair)
+        stacks and of the rect_levels arrays, whose rest is 0).  raw must then be a (ref, cur) pair of stacks.  A
+        sequence that also holds ATANCamera entries aligns lens and ATAN pairs in one call
+        (plsvo_align_raw_any_camera_batch_run): an ATAN pair's frames are not rectified but half-sampled as they are
+        and aligned through the ATAN model; its rect_levels entries are that pyramid."""
+        any_camera = _raw_any_camera(camera, cam_of_pair)
+        rf, batch, keep = (_raw_any_camera_args if any_camera else _raw_call_args)(camera, raw, data, cam_of_pair)
         levels, r = _rect_outputs(camera if cam_of_pair is None else data.cam, rf, data.batch, rect_levels)
         out = abi.AlignOut(data.batch, data.n_segs)
         fn, name = ((self.ctx.lib.plsvo_align_raw_batch_run, "plsvo_align_raw_batch_run") if cam_of_pair is None else
+                    (self.ctx.lib.plsvo_align_raw_any_camera_batch_run, "plsvo_align_raw_any_camera_batch_run") if any_camera else
                     (self.ctx.lib.plsvo_align_raw_multicam_batch_run, "plsvo_align_raw_multicam_batch_run"))
         self.ctx.check(fn(self.ctx.handle, C.byref(rf), C.byref(batch), C.byref(self.params), C.byref(out.struct),
                           C.byref(r) if r is not None else None), name)
@@ -362,11 +367,37 @@ def _raw_call_args(camera, raw, align_data, cam_of_pair=None):
         except ValueError as e:
             raise PlsvoError(str(e)) from None
         chain = False
+    batch, keep_a = _image_free_batch(align_data, chain)
+    return rf, batch, (keep_r, keep_a)
+
+
+def _image_free_batch(align_data, chain: bool):
+    """plsvo_align_batch of the raw-frame calls: no image pointers (the images come from the raw frames)."""
     batch, keep_a = abi.make_align_batch(align_data)
     for l in range(abi.MAX_LEVELS):
         batch.ref_img[l] = batch.cur_img[l] = None
         batch.img_pitch[l] = batch.img_stride[l] = 0
     batch.flags = abi.ALIGN_FRAME_CHAIN if chain else 0
+    return batch, keep_a
+
+
+def _raw_any_camera(camera, cam_of_pair) -> bool:
+    """A raw call with cam_of_pair whose camera sequence holds an ATANCamera: the raw any-camera calls.  A sequence of
+    PinholeCamera only keeps the raw multicam calls."""
+    return cam_of_pair is not None and isinstance(camera, (list, tuple)) and any(isinstance(c, ATANCamera) for c in camera)
+
+
+def _raw_any_camera_args(camera, raw, align_data, cam_of_pair):
+    """plsvo_raw_any_camera_frames and an image-free plsvo_align_batch for the raw any-camera calls: `camera` a sequence
+    of PinholeCamera (distorted lenses) and ATANCamera, indexed by cam_of_pair."""
+    if not all(isinstance(c, (PinholeCamera, ATANCamera)) for c in camera):
+        raise PlsvoError("with cam_of_pair, camera must be a sequence of PinholeCamera and ATANCamera")
+    try:
+        rf, keep_r = abi.make_raw_any_camera_frames(abi.make_raw_cameras(camera), cam_of_pair, raw, align_data.batch,
+                                                    slot=align_data.cam)
+    except ValueError as e:
+        raise PlsvoError(str(e)) from None
+    batch, keep_a = _image_free_batch(align_data, False)
     return rf, batch, (keep_r, keep_a)
 
 
@@ -392,12 +423,13 @@ def track_raw(camera, raw, align_data, poseopt_data, max_level: int = 4, min_lev
               ctx: Context | None = None, rect_levels=None, cam_of_pair=None):
     """track() on raw (distorted) frames, rectified with `camera` on the device (see SparseImgAlign.run_raw for `raw`,
     `rect_levels` and `cam_of_pair`; with cam_of_pair, frame b's errorMultiplier2 is |fx| of its camera and
-    poseopt_data.fx is not used).  Returns (AlignOut, PoseOptOut), plus the dict of rectified levels when rect_levels
-    is given."""
+    poseopt_data.fx is not used; fx_ for an ATANCamera in the sequence, plsvo_track_raw_any_camera_batch_run).
+    Returns (AlignOut, PoseOptOut), plus the dict of rectified levels when rect_levels is given."""
     ctx = ctx or default_context()
     ap = abi.align_params(max_level, min_level, n_iter)
     pp = abi.poseopt_params(reproj_thresh, po_n_iter, -1 if po_n_iter_ref is None else po_n_iter_ref)
-    rf, ab, keep_a = _raw_call_args(camera, raw, align_data, cam_of_pair)
+    any_camera = _raw_any_camera(camera, cam_of_pair)
+    rf, ab, keep_a = (_raw_any_camera_args if any_camera else _raw_call_args)(camera, raw, align_data, cam_of_pair)
     pb, keep_p = abi.make_poseopt_batch(poseopt_data)
     if chained:
         pb.T_f_w = abi._f64p()
@@ -405,6 +437,7 @@ def track_raw(camera, raw, align_data, poseopt_data, max_level: int = 4, min_lev
     ao = abi.AlignOut(align_data.batch, align_data.n_segs)
     po = abi.PoseOptOut(poseopt_data.batch, poseopt_data.n_pts, poseopt_data.n_segs)
     fn, name = ((ctx.lib.plsvo_track_raw_batch_run, "plsvo_track_raw_batch_run") if cam_of_pair is None else
+                (ctx.lib.plsvo_track_raw_any_camera_batch_run, "plsvo_track_raw_any_camera_batch_run") if any_camera else
                 (ctx.lib.plsvo_track_raw_multicam_batch_run, "plsvo_track_raw_multicam_batch_run"))
     ctx.check(fn(ctx.handle, C.byref(rf), C.byref(ab), C.byref(ap), C.byref(pb), C.byref(pp), C.byref(ao.struct), C.byref(po.struct),
                  C.byref(r) if r is not None else None), name)

@@ -112,6 +112,10 @@ struct plsvo_ctx_impl {
   std::vector<double> h_atan_terms;     // [B][4] distortion terms of an ATAN multicam call, staged for the upload
   std::vector<int32_t> h_cam_models;    // [B] model tags of an any-camera call, staged for the upload
   std::vector<RawVisit> h_visit;        // the frames of a raw multicam call in camera-grouped order, with their maps
+  // the table of a raw any-camera call as the raw multicam path reads it: every camera as a lens (an ATAN camera's size
+  // with no parameters) and as a plsvo_match_camera record (a lens as the undistorted pinhole of its fx..cy)
+  std::vector<plsvo_pinhole_camera> h_raw_lens;
+  std::vector<plsvo_match_camera> h_raw_table;
   DevBuf d_visit;
   DevBuf p_out_T;  // every pose-optimiser output, one block
 };
@@ -2470,7 +2474,7 @@ extern "C" int plsvo_last_map_build_ms(plsvo_ctx* ctx, float* ms) {
 
 namespace {
 // The raw frames of one raw call: one camera for every pair (plsvo_raw_frames), or cams[cam_of_pair[b]] for pair b
-// (multicam: plsvo_raw_multicam_frames).
+// (multicam: plsvo_raw_multicam_frames, or plsvo_raw_any_camera_frames with `table`).
 struct RawInput {
   bool multicam;
   const plsvo_pinhole_camera* cams;
@@ -2479,9 +2483,16 @@ struct RawInput {
   const uint8_t* ref_raw;
   const uint8_t* cur_raw;
   size_t pitch, stride;
+  // any-camera: [n_cams] the table as plsvo_match_camera records, whose tags give every camera's model; cams[k] is then
+  // the lens of a PLSVO_CAMERA_PINHOLE camera, and only the size of any other.  NULL: every camera is a lens.
+  const plsvo_match_camera* table = nullptr;
 };
 
-// The cameras of a multicam raw call against the batch.  Nothing is queued here.
+// cams[k] of a raw call is a lens (its frames are rectified), not an ATAN or unknown camera of an any-camera table
+bool is_lens(const RawInput& in, int k) { return !in.table || in.table[k].model == PLSVO_CAMERA_PINHOLE; }
+
+// The cameras of a multicam raw call against the batch: the lenses here; the other cameras of an any-camera table are
+// left to any_camera_check.  Nothing is queued here.
 int raw_multicam_check(plsvo_ctx_impl* c, const RawInput& in, const plsvo_align_batch* ab) {
   if (in.n_cams < 1 || !in.cams || !in.cam_of_pair)
     return fail(c, PLSVO_ERR_INVALID, "raw multicam frames: n_cams must be at least 1, cams and cam_of_pair non-NULL");
@@ -2489,6 +2500,7 @@ int raw_multicam_check(plsvo_ctx_impl* c, const RawInput& in, const plsvo_align_
     return fail(c, PLSVO_ERR_INVALID, "raw multicam frames: PLSVO_ALIGN_FRAME_CHAIN is not supported (a chained frame belongs to two pairs)");
   char msg[160];
   for (int k = 0; k < in.n_cams; ++k) {
+    if (!is_lens(in, k)) continue;
     const plsvo_pinhole_camera& cam = in.cams[k];
     if (cam.width < 1 || cam.height < 1 || cam.width > ab->cam.width || cam.height > ab->cam.height) {
       snprintf(msg, sizeof msg, "raw multicam frames: cams[%d] is %dx%d, batch->cam is %dx%d: every camera must fit inside the batch's image slot",
@@ -2509,11 +2521,15 @@ int raw_multicam_check(plsvo_ctx_impl* c, const RawInput& in, const plsvo_align_
 // PinholeCamera's distortion_ flag: without it undistortImage is a copy
 bool distorted(const plsvo_pinhole_camera& cam) { return fabs(cam.d[0]) > 0.0000001; }
 
+// cams[k] of a raw call has a map: a distorted lens (an ATAN camera's frames are copied whatever its d0, as the pipeline
+// never rectifies FOV frames)
+bool needs_map(const RawInput& in, int k) { return is_lens(in, k) && distorted(in.cams[k]); }
+
 // The maps of a multicam raw call and the order its frames are visited in (c->h_visit).  The cache keeps the maps of
-// the distinct distorted cameras the pairs reference, byte-equal cameras sharing one, and drops the others; a camera
+// the distinct distorted lenses the pairs reference, byte-equal lenses sharing one, and drops the others; a lens
 // already cached is not rebuilt.  Frames [0, B) are the reference frames of the pairs, [B, 2B) the current ones.  The
-// visit order is a counting sort of the frames by map (copied frames last), ascending frame index within a map; each
-// record carries its camera's image size and map pitch.
+// visit order is a counting sort of the frames by map (copied frames last: undistorted lenses and ATAN cameras),
+// ascending frame index within a map; each record carries its camera's image size and map pitch.
 int raw_multicam_maps(plsvo_ctx_impl* c, const RawInput& in, int B, cudaStream_t s) {
   using CamMap = plsvo_ctx_impl::CamMap;
   std::vector<int> slot_of_cam((size_t)in.n_cams, -2);  // -2: not referenced, -1: no distortion, else its map
@@ -2523,7 +2539,7 @@ int raw_multicam_maps(plsvo_ctx_impl* c, const RawInput& in, int B, cudaStream_t
     return [&cam](const plsvo_pinhole_camera& other) { return memcmp(&other, &cam, sizeof cam) == 0; };
   };
   for (int k = 0; k < in.n_cams; ++k) {
-    if (slot_of_cam[k] == -2 || !distorted(in.cams[k])) continue;
+    if (slot_of_cam[k] == -2 || !needs_map(in, k)) continue;
     const auto same = same_as(in.cams[k]);
     auto it = std::find_if(slot_cam.begin(), slot_cam.end(), [&](const plsvo_pinhole_camera* m) { return same(*m); });
     if (it == slot_cam.end()) it = slot_cam.insert(it, &in.cams[k]);
@@ -2584,7 +2600,8 @@ int raw_multicam_maps(plsvo_ctx_impl* c, const RawInput& in, int B, cudaStream_t
 // frames up, the cameras' maps (cached), one rectify + pyramid kernel over every frame storing the levels alignment reads
 // and those rect_out asks for, straight into the device layout of the alignment batch, then the alignment (and
 // pose-optimiser) kernels as the plain upload -> launch -> download sequence runs them, with the multicam kernels and
-// the pairs' own intrinsics for a multicam call.  The arrival-gated streamed path is not taken.
+// the pairs' own intrinsics for a multicam call, or the any-camera kernels and each pair's own model for an any-camera
+// call (its ATAN frames copied into their pyramids, not rectified).  The arrival-gated streamed path is not taken.
 static int raw_run_body(plsvo_ctx* ctx, const RawInput& in, const plsvo_align_batch* ab, const plsvo_align_params* ap,
                         const plsvo_poseopt_batch* pb, const plsvo_poseopt_params* pp, const plsvo_align_result* ao,
                         const plsvo_poseopt_result* po, const plsvo_pyramid_result* rect) {
@@ -2595,6 +2612,12 @@ static int raw_run_body(plsvo_ctx* ctx, const RawInput& in, const plsvo_align_ba
   if (W <= 0 || H <= 0) return fail(c, PLSVO_ERR_INVALID, "raw frames: width and height must be positive");
   if (multicam) {
     if (raw_multicam_check(c, in, ab) != PLSVO_OK) return PLSVO_ERR_INVALID;
+    // any-camera: the table's records against the batch, expanded per pair into c->h_mc_cams, h_atan_terms and
+    // h_cam_models (a lens as the undistorted pinhole of its fx..cy)
+    if (in.table) {
+      const int rc = any_camera_check(c, in.table, in.n_cams, in.cam_of_pair, ab, ap);
+      if (rc != PLSVO_OK) return rc;
+    }
   } else {
     const plsvo_pinhole_camera& cam = in.cams[0];
     if (check_pinhole_params(c, cam, "raw-frame camera") != PLSVO_OK) return PLSVO_ERR_INVALID;
@@ -2634,10 +2657,11 @@ static int raw_run_body(plsvo_ctx* ctx, const RawInput& in, const plsvo_align_ba
     top = std::max(top, l);
   }
   bool distortion = false;
-  for (int k = 0; k < (multicam ? in.n_cams : 1); ++k) distortion = distortion || distorted(in.cams[k]);
+  for (int k = 0; k < (multicam ? in.n_cams : 1); ++k) distortion = distortion || needs_map(in, k);
   if ((multicam ? !undistort_pyramid_multicam_launch : !undistort_pyramid_launch) || (distortion && !undistort_map_launch))
     return fail(c, PLSVO_ERR_CUDA, "raw-frame rectification kernels are not linked into this library", cudaErrorNotSupported);
-  if (multicam && multicam_kernels_present(c, true, pb != nullptr) != PLSVO_OK) return PLSVO_ERR_CUDA;
+  // (any_camera_check has found the any-camera alignment kernels)
+  if (multicam && multicam_kernels_present(c, !in.table, pb != nullptr) != PLSVO_OK) return PLSVO_ERR_CUDA;
   // features, poses, outputs and the host-side sizing of the alignment batch (no image is shipped)
   int rc = plsvo_align_upload(ctx, ab);
   if (rc != PLSVO_OK) return rc;
@@ -2648,15 +2672,18 @@ static int raw_run_body(plsvo_ctx* ctx, const RawInput& in, const plsvo_align_ba
   }
   if (multicam) {
     // pair b is aligned with the undistorted intrinsics and the image size of its camera, and its frame's
-    // errorMultiplier2 is their |fx|
+    // errorMultiplier2 is their |fx|; any-camera: with its camera's model, the records any_camera_check staged, and
+    // errorMultiplier2 |fx| of a lens or fx_ of an ATAN camera (its records' fx)
     c->h_mc_cams.resize(B);
     c->h_po_fx.resize(B);
     for (size_t b = 0; b < B; ++b) {
-      const plsvo_pinhole_camera& k = in.cams[in.cam_of_pair[b]];
-      c->h_mc_cams[b] = plsvo_camera{k.width, k.height, 0, 0, k.fx, k.fy, k.cx, k.cy};
-      c->h_po_fx[b] = fabs(k.fx);
+      if (!in.table) {
+        const plsvo_pinhole_camera& k = in.cams[in.cam_of_pair[b]];
+        c->h_mc_cams[b] = plsvo_camera{k.width, k.height, 0, 0, k.fx, k.fy, k.cx, k.cy};
+      }
+      c->h_po_fx[b] = fabs(c->h_mc_cams[b].fx);
     }
-    rc = multicam_select(c, c->h_mc_cams.data());
+    rc = in.table ? any_camera_select(c) : multicam_select(c, c->h_mc_cams.data());
     if (rc == PLSVO_OK && pb) rc = poseopt_fx_select(c, c->h_po_fx.data());
     if (rc != PLSVO_OK) return rc;
   }
@@ -2758,6 +2785,31 @@ RawInput raw_input(const plsvo_raw_frames* raw) {
 RawInput raw_input(const plsvo_raw_multicam_frames* raw) {
   return RawInput{true, raw->cams, raw->n_cams, raw->cam_of_pair, raw->ref_raw, raw->cur_raw, raw->pitch, raw->stride};
 }
+// The table of an any-camera call as the raw multicam path reads it (c->h_raw_lens, c->h_raw_table); a NULL or empty
+// table is passed on as NULL for raw_multicam_check to reject.  An unknown model keeps its tag for any_camera_check.
+RawInput raw_input(plsvo_ctx_impl* c, const plsvo_raw_any_camera_frames* raw) {
+  const bool table = raw->cams && raw->n_cams >= 1;
+  const size_t K = table ? (size_t)raw->n_cams : 0;
+  c->h_raw_lens.assign(K, plsvo_pinhole_camera{});
+  c->h_raw_table.assign(K, plsvo_match_camera{});
+  for (size_t k = 0; k < K; ++k) {
+    const plsvo_raw_camera& r = raw->cams[k];
+    plsvo_match_camera& m = c->h_raw_table[k];
+    m.model = r.model;
+    if (r.model == PLSVO_CAMERA_PINHOLE) {
+      const plsvo_pinhole_camera& l = r.pinhole;
+      c->h_raw_lens[k] = l;
+      m.pinhole = plsvo_camera{l.width, l.height, 0, 0, l.fx, l.fy, l.cx, l.cy};
+    } else {
+      c->h_raw_lens[k].width = r.atan.width, c->h_raw_lens[k].height = r.atan.height;
+      m.atan = r.atan;
+    }
+  }
+  RawInput in{true, table ? c->h_raw_lens.data() : nullptr, raw->n_cams, raw->cam_of_pair, raw->ref_raw, raw->cur_raw,
+              raw->pitch, raw->stride};
+  in.table = table ? c->h_raw_table.data() : nullptr;
+  return in;
+}
 }  // namespace
 
 extern "C" int plsvo_align_raw_batch_run(plsvo_ctx* ctx, const plsvo_raw_frames* raw, const plsvo_align_batch* b,
@@ -2787,6 +2839,22 @@ extern "C" int plsvo_track_raw_multicam_batch_run(plsvo_ctx* ctx, const plsvo_ra
                                                   const plsvo_poseopt_result* po, const plsvo_pyramid_result* rect_out) {
   if (!ctx || !raw || !ab || !ap || !pb || !pp || !po) return PLSVO_ERR_INVALID;
   return settled(CTX(ctx), raw_run_body(ctx, raw_input(raw), ab, ap, pb, pp, ao, po, rect_out));
+}
+
+extern "C" int plsvo_align_raw_any_camera_batch_run(plsvo_ctx* ctx, const plsvo_raw_any_camera_frames* raw,
+                                                    const plsvo_align_batch* b, const plsvo_align_params* p,
+                                                    const plsvo_align_result* o, const plsvo_pyramid_result* rect_out) {
+  if (!ctx || !raw || !b || !p || !o) return PLSVO_ERR_INVALID;
+  return settled(CTX(ctx), raw_run_body(ctx, raw_input(CTX(ctx), raw), b, p, nullptr, nullptr, o, nullptr, rect_out));
+}
+
+extern "C" int plsvo_track_raw_any_camera_batch_run(plsvo_ctx* ctx, const plsvo_raw_any_camera_frames* raw,
+                                                    const plsvo_align_batch* ab, const plsvo_align_params* ap,
+                                                    const plsvo_poseopt_batch* pb, const plsvo_poseopt_params* pp,
+                                                    const plsvo_align_result* ao, const plsvo_poseopt_result* po,
+                                                    const plsvo_pyramid_result* rect_out) {
+  if (!ctx || !raw || !ab || !ap || !pb || !pp || !po) return PLSVO_ERR_INVALID;
+  return settled(CTX(ctx), raw_run_body(ctx, raw_input(CTX(ctx), raw), ab, ap, pb, pp, ao, po, rect_out));
 }
 
 extern "C" int plsvo_match_direct_batch_run(plsvo_ctx* ctx, const plsvo_match_batch* in, const plsvo_match_result* out) {

@@ -832,6 +832,52 @@ def make_raw_multicam_batch(cams, dists, cam_of_pair, n_pts: int = 300, n_segs: 
     return out[:-1] + ((ref, cur),) + out[-1:]
 
 
+def make_raw_any_camera_batch(cams, cam_of_pair, slot: Camera | None = None, fill=0, poseopt: bool = False, n_pts: int = 300,
+                              n_segs: int = 80, seed: int = 3000, scene: Scene | None = None, **align_kw):
+    """A batch of raw pairs from distorted lenses (api.PinholeCamera) and ATAN (FOV) cameras (api.ATANCamera), of one size
+    or several, for the raw any-camera calls.  A lens pair is make_raw_multicam_batch's: features, poses, ground truth and
+    pyramids of the undistorted camera (the lens's size and fx..cy), its raw frames rendered through the lens
+    (render_distorted).  An ATAN pair is make_any_camera_batch's, its raw frames the level 0 it renders through its model
+    (the pipeline does not rectify FOV frames).  The per-camera parts and raw stacks are padded into one slot with
+    merge_sizes (slot, fill as there).  Returns (AlignData, (ref_raw, cur_raw) u8 [B, H, W], parts, groups), or
+    (AlignData, PoseOptData, raw, parts, po_parts, groups) when `poseopt`: parts[i] and groups[i] those of the i-th camera
+    that has pairs.  The pose optimiser of frame b then takes errorMultiplier2 = |fx| of a lens, fx_ of an ATAN camera."""
+    scene = scene or Scene()
+    cam_of_pair = np.asarray(cam_of_pair)
+    dev = torch.device(align_kw.get("device", "cpu"))
+    groups = [np.flatnonzero(cam_of_pair == k) for k in range(len(cams))]
+    used = [k for k in range(len(cams)) if len(groups[k])]
+    al_parts, po_parts, raws = [], [], []
+    for k in used:
+        a = cams[k]
+        atan = a if hasattr(a, "fx_") else None
+        if atan is not None:
+            cam = Camera(a.width, a.height, a.fx_, a.fy_, a.cx_, a.cy_)
+        else:
+            s = a.struct
+            cam, dist = Camera(s.width, s.height, s.fx, s.fy, s.cx, s.cy), tuple(s.d)
+        kw = dict(cam=cam, batch=len(groups[k]), n_pts=n_pts, n_segs=n_segs, seed=seed + 104729 * k, scene=scene, atan=atan,
+                  **align_kw)
+        if poseopt:
+            al, po = make_track_batch(**kw)
+            po.fx = a.errorMultiplier2() if atan is not None else abs(cam.fx)
+            po_parts.append(po)
+        else:
+            al = make_align_batch(**kw)
+        al_parts.append(al)
+        pair = []
+        for poses in (al.T_ref_w, al.T_cur_w_gt):
+            pose = torch.tensor(poses, dtype=torch.float64, device=dev)
+            img = scene.render(cam, pose, atan=atan) if atan is not None else render_distorted(scene, cam, dist, pose)
+            pair.append(np.ascontiguousarray(img.cpu().numpy()))
+        raws.append(tuple(pair))
+    index = [groups[k] for k in used]
+    al, _, raw = merge_sizes(al_parts, index, slot=slot, fill=fill, raws=raws)
+    if not poseopt:
+        return al, raw, al_parts, index
+    return al, scatter_batches(po_parts, index, len(cam_of_pair)), raw, al_parts, po_parts, index
+
+
 def run_sequence(poses, steps, track_fn):
     """The frame-to-frame chain of FrameHandlerMono::processFrame (src/frame_handler_mono.cpp:263-340) over a sequence:
     new_frame.T_f_w = last_frame.T_f_w (:266), sparse image alignment, pose optimisation, and the result becomes the
